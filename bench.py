@@ -9,10 +9,10 @@ shape (lock_fasst/caladan/trace_init.sh: 24,000,000 lock ids, uniform, 5-10 ids 
 0.2) driven closed-loop by 1,048,576 logical clients through the FaSST protocol of lock_fasst/caladan/client.cc
 against a 36,000,000-slot lock table ("REF" in SURVEY.md 8(d)).  One STEP = one batch of 4 client rounds =
 4,194,304 wire requests.  W + K steps of the closed loop are recorded (every reply of the recording is compared with
-the UNMODIFIED reference server binary fed the same stream); the timed region replays the K recorded steps, device
-resident, in cycles -- the server state is restored from a snapshot at the start of every cycle (inside the timed
-region) so that every cycle reproduces the recording bit for bit -- until it is at least one second long.  Every step
-reads a different 37.7 MB trace segment (K segments >> L2).  At N > 1 every rank drives its own 1,048,576 clients and
+the UNMODIFIED reference server binary fed the same stream); the timed region replays the K recorded steps once,
+device resident, from the server state the W warm-up steps left, and must reproduce the recording bit for bit.  Every
+step reads a different 37.7 MB trace segment (K segments >> L2).  --dump-outputs DIR writes the replies of the last
+timed step (a fixed sample of 2^20 of them) as DIR/reply_*.npy.  At N > 1 every rank drives its own 1,048,576 clients and
 the key space grows with N (36 M slots and 24 M ids PER GPU: constant contention), requests travel to the owning GPU
 through the dispatch / engine / combine step over NVLink; the reference's fixed 36 M / 24 M constants at N > 1, TATP
 and SmallBank on the reference's shard placement, HOT, store GET, lock_2pl, log_server and the UDP front-end are
@@ -36,7 +36,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 CLIENTS = 1 << 20
 ROUNDS_PER_STEP = 4
 STEP_REQS = CLIENTS * ROUNDS_PER_STEP
-TIMED_SECONDS = float(os.environ.get("DINT_BENCH_SECONDS", "1.0"))      # minimum length of every timed region
+TIMED_SECONDS = float(os.environ.get("DINT_BENCH_SECONDS", "1.0"))      # minimum length of the end-to-end and side timed regions
 # algorithmic bytes per request (SURVEY.md 8(d)): wire in + wire out + state at the reference's field granularity
 FASST_BYTES = {4: 22, 5: 26, 6: 22, 7: 22, 8: 30}          # by reply type
 STORE_GET_BYTES = 186
@@ -48,7 +48,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
@@ -177,17 +177,10 @@ def fasst_alg_bytes(resps, msg=9):
     return int(sum(FASST_BYTES[t] * int(cnt[t]) for t in FASST_BYTES)), {str(t): int(cnt[t]) for t in FASST_BYTES}
 
 
-def cycles_for(step_ms, k):
-    return max(1, int(np.ceil(TIMED_SECONDS * 1e3 / max(step_ms * k, 1e-6))))
-
-
-def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=True, timed_seconds=None):
+def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=True):
     """N = 1.  Returns the result dict main() turns into the JSON line."""
     from dint_b200 import Engine, PinnedBuffer, wire
     from dint_b200.workloads import Workload
-    global TIMED_SECONDS
-    if timed_seconds is not None:
-        saved, TIMED_SECONDS = TIMED_SECONDS, timed_seconds
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     n_steps, msg = steps + warmup, 9
     rq_pin, rs_pin = PinnedBuffer(CLIENTS * msg), PinnedBuffer(CLIENTS * msg)
@@ -215,25 +208,20 @@ def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=Tru
             eng.submit_tensor(d_req[s], d_out[0])
         torch.cuda.synchronize(dev)
         ok = bool((d_out[0].cpu().numpy() == resps[warmup - 1]).all()) if warmup else True
-        snap = eng.snapshot()                    # the state every cycle starts from
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ev[0].record(stream)
-        for s in range(steps):                   # one untimed cycle: sizes the timed region, warms everything
+        snap = eng.snapshot()                    # the state the timed steps start from
+        for s in range(steps):                   # one untimed pass warms every kernel and buffer
             eng.submit_tensor(d_req[warmup + s], d_out[s])
-        ev[1].record(stream)
-        torch.cuda.synchronize(dev)
-        cycles = cycles_for(ev[0].elapsed_time(ev[1]) / steps, steps)
+        eng.restore(snap, stream.cuda_stream)
         eng.reset_stats()
-        eng.profile(Engine.PROF_APPLY)           # events around the dominant kernel only (all-kernel profiling costs ~20 %)
+        eng.profile(Engine.PROF_APPLY)           # events around the dominant kernel only (all-kernel profiling costs more)
         sampler = ClockSampler(dev.index)
         sampler.start()
         time.sleep(0.01)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
         torch.cuda.synchronize(dev)
         ev[0].record(stream)
-        for _ in range(cycles):
-            eng.restore(snap, stream.cuda_stream)                # inside the timed region
-            for s in range(steps):
-                eng.submit_tensor(d_req[warmup + s], d_out[s])
+        for s in range(steps):
+            eng.submit_tensor(d_req[warmup + s], d_out[s])
         ev[1].record(stream)
         torch.cuda.synchronize(dev)
         ms = ev[0].elapsed_time(ev[1])
@@ -241,8 +229,9 @@ def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=Tru
         eng.profile(False)
         kt, st = eng.kernel_times(), eng.stats()
         n_bad = sum(0 if bool((d_out[s].cpu().numpy() == resps[warmup + s]).all()) else 1 for s in range(steps))
-        out.update(ms=ms, cycles=cycles, kernel_times=kt, stats=st, clocks=clocks, parity_replay=(ok and n_bad == 0))
-        # a fully profiled cycle (not the timed one) for the per-kernel breakdown
+        out.update(ms=ms, kernel_times=kt, stats=st, clocks=clocks, parity_replay=(ok and n_bad == 0),
+                   last_replies=d_out[steps - 1].cpu().numpy())
+        # a fully profiled pass (not the timed one) for the per-kernel breakdown
         eng.reset_stats()
         eng.profile(True)
         eng.restore(snap, stream.cuda_stream)
@@ -253,9 +242,9 @@ def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=Tru
         out["all_kernel_times"] = eng.kernel_times()
         eng.free_snapshot(snap)
         del d_req, d_out
-    out.update(committed=sum(committed[warmup:]) * cycles, requests=steps * STEP_REQS * cycles, steps_timed=steps * cycles)
+    out.update(committed=sum(committed[warmup:]), requests=steps * STEP_REQS, steps_timed=steps)
     alg, mix = fasst_alg_bytes(resps[warmup:])
-    out.update(alg_bytes=alg * cycles, reply_mix=mix)
+    out.update(alg_bytes=alg, reply_mix=mix)
     # ---- end to end through the host-facing C ABI call (pinned host buffers, H2D + D2H inside) ----
     if do_e2e:
         with Engine(wire.FASST, device=dev.index, chunk=args.chunk) as eng:
@@ -282,8 +271,6 @@ def run_fasst(args, torch, fam_name, fam, steps, warmup, do_e2e=True, do_ref=Tru
                        e2e_committed=sum(committed[warmup:]) * (n_e2e // steps), e2e_requests=STEP_REQS * n_e2e)
     if ref_bg is not None:
         out["cpu_baseline"] = ref_bg.get(timeout=600)
-    if timed_seconds is not None:
-        TIMED_SECONDS = saved
     out["first_step"] = (reqs[0], resps[0], txn_per_req)
     return out
 
@@ -355,26 +342,19 @@ def run_fasst_sharded(args, torch, dist, rank, world, scaled, steps, warmup, do_
     torch.cuda.synchronize(dev)
     dist.barrier()
     snap = se.engine.snapshot()
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    ev[0].record(stream)
-    for s in range(steps):
+    for s in range(steps):                               # one untimed pass warms every kernel and buffer
         step(warmup + s, s)
-    ev[1].record(stream)
-    torch.cuda.synchronize(dev)
-    t = torch.tensor([ev[0].elapsed_time(ev[1]) / steps], device=dev, dtype=torch.float64)
-    dist.all_reduce(t, op=dist.ReduceOp.MAX)
-    cycles = cycles_for(float(t[0]), steps)
+    se.engine.restore(snap, stream.cuda_stream)          # local state, ordered on the engine's stream between two batches
     se.engine.reset_stats()
     se.engine.profile(se.engine.PROF_APPLY)
     sampler = ClockSampler(dev.index)
     sampler.start()
-    dist.barrier()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     torch.cuda.synchronize(dev)
+    dist.barrier()
     ev[0].record(stream)
-    for _ in range(cycles):
-        se.engine.restore(snap, stream.cuda_stream)          # local state, ordered on the engine's stream between two batches
-        for s in range(steps):
-            step(warmup + s, s)
+    for s in range(steps):
+        step(warmup + s, s)
     ev[1].record(stream)
     torch.cuda.synchronize(dev)
     dist.barrier()
@@ -386,10 +366,11 @@ def run_fasst_sharded(args, torch, dist, rank, world, scaled, steps, warmup, do_
         got = torch.cat(last[s]).cpu().numpy()
         n_bad += 0 if bool((got == resps[warmup + s]).all()) else 1
     ok = n_bad == 0 and se.check_p2p() == (0, 0) and flags_rec == (0, 0)
-    out = dict(ms=ms, cycles=cycles, kernel_times=se.engine.kernel_times(), stats=se.engine.stats(), clocks=clocks, parity_replay=ok,
-               committed=sum(committed[warmup:]) * cycles, requests=steps * STEP_REQS * cycles, steps_timed=steps * cycles, wl_stats=wl_stats)
+    out = dict(ms=ms, kernel_times=se.engine.kernel_times(), stats=se.engine.stats(), clocks=clocks, parity_replay=ok,
+               committed=sum(committed[warmup:]), requests=steps * STEP_REQS, steps_timed=steps, wl_stats=wl_stats,
+               last_replies=torch.cat(last[steps - 1]).cpu().numpy())
     alg, mix = fasst_alg_bytes(resps[warmup:])
-    out.update(alg_bytes=alg * cycles, reply_mix=mix)
+    out.update(alg_bytes=alg, reply_mix=mix)
     se.engine.free_snapshot(snap)
     se.close()
     del d_req
@@ -762,7 +743,7 @@ def run_store_get(args, torch, rank, steps, warmup):
                         "frac_with_this_engines_64B_entry": ach170 / peak,
                         "note": "186 B/GET is SURVEY 8(d)'s figure (reference 4-key entry); with this engine's one-key 64-byte entry the "
                                 "minimum is 53 + 53 + 64 = 170 B/GET",
-                        "traffic": load_static_traffic("k_apply<store>")}}
+                        "traffic": None}}
     if bg is not None:
         res["cpu_baseline"] = bg.get(timeout=400)
     return res
@@ -819,36 +800,28 @@ def run_txn(args, torch, rank, kind_name, rounds_timed=12, rounds_warm=8, client
             if d[r][s_].numel():
                 engs[s_].submit_tensor(d[r][s_], outs[r][s_])
     torch.cuda.synchronize(dev)
-    snaps = [e.snapshot() for e in engs]
-    stream = torch.cuda.current_stream(dev)
     for e in engs:
         e.reset_stats()
-    total_ms, cycles = 0.0, 0
-    while total_ms < min(TIMED_SECONDS, 0.5) * 1e3 and cycles < 200:
-        for e, sn in zip(engs, snaps):
-            e.restore(sn, stream.cuda_stream)                  # outside the timed region (GBs of tables)
-        torch.cuda.synchronize(dev)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for r in range(rounds_warm, rounds_warm + rounds_timed):
-            for s_ in range(G):
-                if d[r][s_].numel():
-                    engs[s_].submit_tensor(d[r][s_], outs[r][s_])
-        e1.record()
-        torch.cuda.synchronize(dev)
-        total_ms += e0.elapsed_time(e1)
-        cycles += 1
+    # one timed pass: three TATP shards hold 45 GB, so a device snapshot of each (to repeat the pass) would not fit 80 GB
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for r in range(rounds_warm, rounds_warm + rounds_timed):
+        for s_ in range(G):
+            if d[r][s_].numel():
+                engs[s_].submit_tensor(d[r][s_], outs[r][s_])
+    e1.record()
+    torch.cuda.synchronize(dev)
+    total_ms = e0.elapsed_time(e1)
     ok = all(bool((outs[r][s_].cpu().numpy() == rec[r][1][s_]).all()) for r in range(rounds_warm, rounds_warm + rounds_timed) for s_ in range(G))
     launches = sum(e.stats()["kernel_launches"] for e in engs)
     conflicted = sum(e.stats()["conflicted"] for e in engs)
-    for e, sn in zip(engs, snaps):
-        e.free_snapshot(sn)
+    for e in engs:
         e.close()
-    tc = sum(committed[rounds_warm:]) * cycles
-    tr = sum(nreq[rounds_warm:]) * cycles
+    tc = sum(committed[rounds_warm:])
+    tr = sum(nreq[rounds_warm:])
     res = {"workload": f"{kind_name} mix, {clients} closed-loop clients, 3 shard servers x {subscribers} "
                        f"{'subscribers' if kind == wire.TATP else 'accounts'} on one GPU, "
-                       f"{rounds_timed} protocol rounds x {cycles} cycles timed (device-resident replay of the recorded closed-loop trace, state restored between cycles)",
+                       f"{rounds_timed} protocol rounds timed once (device-resident replay of the recorded closed-loop trace)",
            "abort_rate": 1.0 - st["committed"] / max(1, st["txns"]), "timed_region_s": total_ms * 1e-3,
            "txn_per_s": tc / (total_ms * 1e-3), "requests_per_s": tr / (total_ms * 1e-3), "requests_per_txn": st["requests"] / max(1, st["txns"]),
            "commit_rate_by_type": {k: round(v[1] / max(1, v[0]), 4) for k, v in st["by_type"].items()},
@@ -877,26 +850,36 @@ class Watchdog:
         self.t.cancel()
 
 
-def load_static_traffic(name):
-    """dram__bytes_read + dram__bytes_write per launch of the named kernel from the committed ncu capture (profiles/):
-    a STATIC figure measured once per round, not by this run."""
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if not os.path.exists(tp):
-        return None
-    return json.load(open(tp)).get(name)
+def dump_outputs(out_dir, replies, sample=1 << 20):
+    """The lock_fasst replies of the last timed step (rank 0's at N > 1), field by field: reply_type (float32), reply_lid and
+    reply_ver (float64, exact for u32), and reply_index, the positions of the replies in the step.  A step of more than
+    `sample` replies is cut to a fixed, seeded sample of that many positions (28 MB in all)."""
+    from dint_b200 import wire
+    rec = wire.as_records(wire.FASST, replies)
+    idx = np.arange(len(rec))
+    if len(rec) > sample:
+        idx = np.sort(np.random.default_rng(0).choice(len(rec), size=sample, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "reply_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "reply_type.npy"), rec["type"][idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "reply_lid.npy"), rec["lid"][idx].astype(np.float64))
+    np.save(os.path.join(out_dir, "reply_ver.npy"), rec["ver"][idx].astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (4,194,304 requests each)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="dint_b200", choices=["dint_b200", "reference"])
     ap.add_argument("--chunk", type=int, default=1 << 20)
     ap.add_argument("--no-extra", action="store_true", help="skip the side measurements")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the replies of the last timed step to DIR/*.npy")
     ap.add_argument("--extra-only", default=None, help=argparse.SUPPRESS)     # child-process mode for a side measurement
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.extra_only:
         import torch
         print(json.dumps(run_closed_loop_extra(args, torch, 0, args.extra_only)), flush=True)
@@ -928,6 +911,8 @@ def main():
         res = run_fasst_sharded(args, torch, dist, rank, world, True, args.steps, args.warmup)
     else:
         res = run_fasst(args, torch, "REF", REF, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res.pop("last_replies"))
 
     # reduce over ranks: time = max, work = sum
     ms, committed, reqs = res["ms"], res["committed"], res["requests"]
@@ -995,8 +980,7 @@ def main():
     achieved = alg_per_launch / avg_s / 1e9
     akt = res.get("all_kernel_times", kt)
     roof = {"kernel": "k_apply<lock_fasst>", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": load_static_traffic("k_apply<lock_fasst>"),
-            "traffic_source": "static: profiles/ncu_traffic.json (one single-pass ncu capture per round, --cache-control none; not measured by this run)",
+            "traffic": None, "traffic_source": "not measured: DRAM byte counts need a profiler capture, which this run does not take",
             "peak_source": peak_how, "avg_launch_us": avg_s * 1e6, "launches": nl, "algorithmic_bytes_per_launch": alg_per_launch,
             "timing": "CUDA events around every k_apply launch of the timed region",
             "whole_step": {"achieved": alg_total / (ms * 1e-3) / 1e9 / world, "frac": alg_total / (ms * 1e-3) / 1e9 / world / peak,
@@ -1004,25 +988,24 @@ def main():
             "all_kernels_ms_profiled_cycle": {k: round(v[1], 3) for k, v in akt.items()}}
     if "k_classify" in akt:
         l1, t1 = akt["k_classify"]
-        ach1 = (res["alg_bytes"] / res["cycles"]) / max(1, l1) / (t1 / l1 * 1e-3) / 1e9 if world == 1 else None
+        ach1 = res["alg_bytes"] / max(1, l1) / (t1 / l1 * 1e-3) / 1e9 if world == 1 else None
         roof["k_classify"] = {"avg_launch_us": t1 / l1 * 1e3, "launches_profiled_cycle": l1,
                               "achieved_same_algorithmic_bytes": ach1, "frac": (ach1 / peak) if ach1 else None,
                               "note": "second pass over the same requests (conflict flags + replay of the previous chunk): it moves no algorithmic byte "
-                                      "of its own, so its fraction is quoted against the step's algorithmic bytes; from the fully profiled cycle, not the timed one"}
+                                      "of its own, so its fraction is quoted against the step's algorithmic bytes; from the fully profiled pass, not the timed one"}
     line = {
         "metric": "committed txns/sec (lock_fasst)", "value": committed / (ms * 1e-3), "unit": "txn/s",
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / res["steps_timed"],
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32", "data": "synthetic",
         "config": {"workload": WORKLOAD + (f" -- per GPU; key space scaled with the GPU count: {36 * world},000,000 slots, {24 * world},000,000 ids in total "
                                            "(constant contention; the reference's fixed constants: extra.lock_fasst_reference_constants)" if world > 1 else ""),
-                   "baseline_config": "BASELINE.json configs[1] (lock_fasst OCC validate/commit, 1 B200).  Its '4800 keys, "
+                   "baseline_config": "BASELINE.json configs[1] (lock_fasst OCC validate/commit, 1 GPU).  Its '4800 keys, "
                                       "Zipf-0.8, 24M-op' wording is, in the reference, 4800 trace FILES, read fraction 0.8 and 24 M "
                                       "uniform lock ids (BASELINE.md section 1 note, lock_fasst/caladan/trace_init.sh:9-27): the headline "
                                       "runs that reference shape; the literal reading (4800 ids, Zipf 0.8) is extra.lock_fasst_HOT",
                    "requests_per_step": STEP_REQS * world, "chunk": args.chunk,
-                   "timed_region": f"{res['cycles']} cycles x {args.steps} recorded steps = {res['steps_timed']} steps, {ms * 1e-3:.3f} s; the server state is "
-                                   "restored from a snapshot at the start of every cycle INSIDE the timed region",
-                   "cache": "every step replays a different 37.7 MB trace segment (K segments larger than L2; lock/version tables 148.5 MB > 126 MB L2)",
+                   "timed_region": f"{res['steps_timed']} recorded steps replayed once, {ms * 1e-3:.3f} s",
+                   "cache": "every step replays a different 37.7 MB trace segment (K segments larger than L2; lock/version tables 148.5 MB > 50 MB L2)",
                    "parallelism": (f"key-space sharded x{world}: dispatch / engine / combine kernels over NVLink peer memory (owner = slot % {world}), "
                                    "one process per GPU") if world > 1 else "single GPU"},
         "requests_per_s": reqs / (ms * 1e-3),
@@ -1059,7 +1042,7 @@ def main():
         line["cpu_baseline"].pop("gpu_replies_equal_reference", None)
     if not args.no_extra and world == 1:
         try:
-            hot = run_fasst(args, torch, "HOT", HOT, max(3, args.steps // 3), 3, do_e2e=False, do_ref=True, timed_seconds=min(TIMED_SECONDS, 0.5))
+            hot = run_fasst(args, torch, "HOT", HOT, max(3, args.steps // 3), 3, do_e2e=False, do_ref=True)
             extra["lock_fasst_HOT"] = {
                 "workload": "BASELINE.json literal: 4800 lock ids, Zipf 0.8, same clients/protocol",
                 "txn_per_s": hot["committed"] / (hot["ms"] * 1e-3), "requests_per_s": hot["requests"] / (hot["ms"] * 1e-3),

@@ -1,4 +1,4 @@
-"""dint_b200 -- B200-resident batched implementation of DINT's per-request server hot path.
+"""dint_b200 -- GPU-resident (H100) batched implementation of DINT's per-request server hot path.
 
     from dint_b200 import Engine, wire
     eng = Engine(wire.FASST)            # stands in for `lock_fasst/udp/server 1`

@@ -1,6 +1,6 @@
 """In-tree build of the native libraries (no JIT cache: the .so files travel with the repo snapshot).
 
-  dint_b200/lib/libdint_b200.so   CUDA kernels + C ABI (include/dint_b200.h), nvcc, sm_100a only
+  dint_b200/lib/libdint_b200.so   CUDA kernels + C ABI (include/dint_b200.h), nvcc, sm_90a (H100) only
   dint_b200/lib/libdint_wl.so     workload clients (CPU C++: the reference's closed-loop clients restated)
   dint_b200/lib/dint_udp_server   the reference's UDP server front-end over the C ABI (recvmmsg / sendmmsg)
 """
@@ -17,7 +17,7 @@ LIB = os.path.join(LIBDIR, f"libdint_b200_{_TAG}.so" if _TAG else "libdint_b200.
 WL_LIB = os.path.join(LIBDIR, "libdint_wl.so")
 UDP_SERVER = os.path.join(LIBDIR, "dint_udp_server")
 
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -43,6 +43,9 @@ def find_nvcc():
 
 
 def build(force=False, verbose=False):
+    if not force and os.path.isdir(LIBDIR) and not os.access(LIBDIR, os.W_OK) and \
+            all(os.path.exists(p) for p in (LIB, WL_LIB, UDP_SERVER)):
+        return LIB                    # a read-only tree: use the libraries it was built with
     os.makedirs(LIBDIR, exist_ok=True)
     cu_src = _sources((".cu", ".cuh", ".h"))
     if force or _newer(LIB, cu_src):

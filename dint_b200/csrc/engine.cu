@@ -87,8 +87,8 @@ struct dint_engine {
   uint32_t route_tiles = 0;
   uint32_t* d_route2 = nullptr;              // dispatch scratch: counters, totals, look-back descriptors
   uint32_t route_desc_tiles = 0, route_seq = 0;
-  int grid_route = 148 * 4;                  // CTAs of k_route_dispatch: 4 per SM are resident (64 registers x 256 threads); 2^20 small
-                                             // records = 512 tiles = ONE wave (tiles are drawn by ticket, so any grid is correct)
+  int grid_route = 0;                        // CTAs of k_route_dispatch: 4 per SM are resident (64 registers x 256 threads)
+                                             // (tiles are drawn by ticket, so any grid is correct)
   // L2 persistence: the flag sets (+ lock_fasst lock bits) live in one arena that every launch maps
   // with a persisting access-policy window, so the streaming request/reply traffic cannot evict it
   uint8_t* hot_arena = nullptr;
@@ -226,6 +226,8 @@ template <int KIND, bool HAS_LOG>
 static int grids_for(dint_engine* e) {
   int per_sm = 0, sms = 0;
   CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
+  e->sms = sms;
+  e->grid_route = 4 * sms;
   e->smem_stage = Stage<Wire<KIND>::MSG>::N * Stage<Wire<KIND>::MSG>::BYTES;
   if (e->smem_stage > 48 * 1024) {
     CU(cudaFuncSetAttribute(k_classify<KIND, HAS_LOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_stage));
@@ -244,7 +246,6 @@ static int grids_for(dint_engine* e) {
   if (per_sm < 1) return set_err(DINT_EIO, "k_ordered cannot be resident");
   if (per_sm > 4) per_sm = 4;
   e->coop_grid = per_sm * sms;
-  e->sms = sms;
   return DINT_OK;
 }
 
@@ -334,8 +335,8 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
     N.entries = (uint8_t*)fresh;
     {
       ProfScope ps(e, s, KT_LOAD);
-      if (e->kind == DINT_SMALLBANK) k_kv_rehash<8><<<148 * 8, 256, 0, s>>>(T, N);
-      else k_kv_rehash<40><<<148 * 8, 256, 0, s>>>(T, N);
+      if (e->kind == DINT_SMALLBANK) k_kv_rehash<8><<<e->sms * 8, 256, 0, s>>>(T, N);
+      else k_kv_rehash<40><<<e->sms * 8, 256, 0, s>>>(T, N);
     }
     CU(cudaStreamSynchronize(s));
     for (auto& p : e->allocs) if (p == (void*)T.entries) p = fresh;
@@ -458,7 +459,7 @@ template <int MSG>
 static int route_combine_t(dint_engine* e, const RouteArgs& a, cudaStream_t s) {
   using RT = RTile<MSG>;
   int grid = (int)a.n_tiles;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > e->grid_route) grid = e->grid_route;
   k_route_combine<MSG><<<grid, kThreads, RT::SMEM, s>>>(a);
   CU(cudaGetLastError());
   return DINT_OK;
@@ -666,7 +667,7 @@ int dint_create(int kind, const dint_cfg* cfg, int device, dint_engine** out) {
   if (cf.chunk == 0) cf.chunk = 1u << 20;
   e->chunk = (cf.chunk + kTile - 1) / kTile * kTile;
   {
-    // host-path slice schedule (measured, tools/e2e_probe.py round 1: every schedule between 128 K and 1 M lands within 5 %)
+    // host-path slice schedule: 128 K requests doubling up to 256 K (see dint_submit)
     const uint32_t want = 1u << 18;
     e->host_chunk = want < e->chunk ? want : e->chunk;
     e->host_min_slice = 131072u;
@@ -873,8 +874,6 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
   const uint8_t* rq = (const uint8_t*)req;
   uint8_t* rs = (uint8_t*)resp;
   unsigned long long err_before = e->stats.errors;
-  // (Zero-copy replies -- K2 storing straight into pinned host memory instead of a D2H stage -- were measured in
-  // round 2 and dropped: 1.42 vs 1.73 G req/s at 2^20 requests per call, profiles/r02_variants.md.)
   // three-stage pipeline: H2D (s_in) | kernels (stream) | D2H (s_out).  Slice k's replies are final only
   // after the launch that replays its listed requests -- K1 of slice k+1, or the flush after the last
   // slice -- so D2H(k) is ordered behind that.
@@ -888,13 +887,9 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
     CU(cudaEventRecord(e->ev_out[pb], e->s_out));
     return DINT_OK;
   };
-  // Slice schedule.  PCIe moves large copies better than small ones (B200 box, pinned, both directions busy:
-  // 37 GB/s per direction at 2.4 MB, 46 at 9.4 MB, 50 at 38 MB: tools/pcie_probe.cu), but the first slice's
-  // H2D and the last two slices' kernels + D2H overlap with nothing.  So a call is cut as a pyramid: slices
-  // double from host_min_slice up to host_chunk, stay there, and halve back down at the end.  (Measured with
-  // tools/e2e_probe.py: every schedule between 128K..1M slices lands within 5 % -- the copies, not the
-  // kernels or the launches (11 us of CPU per slice), are the bound: 1M requests = 345 us vs 203 us for two
-  // perfectly overlapped 9.4 MB copies.)
+  // Slice schedule.  PCIe moves large copies better than small ones (tools/pcie_probe.cu measures it), but the
+  // first slice's H2D and the last two slices' kernels + D2H overlap with nothing.  So a call is cut as a
+  // pyramid: slices double from host_min_slice up to host_chunk, stay there, and halve back down at the end.
   HostSlices sched(n, e->host_min_slice, hchunk, e->host_ramp_up);
   uint64_t off = 0;
   for (uint64_t cn; (cn = sched.next()) != 0; k++) {

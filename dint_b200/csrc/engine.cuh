@@ -10,8 +10,8 @@
 //                 A (the versioned data: ver_table entry / KV rows) and L (the lock word / counters).
 //                 A request is a reader of A (RA), a writer of A (WA) and/or a writer of L (WL); the
 //                 nibble holds R (an RA exists), WA, WL and W2 (two or more writers of one class).
-//                 The flag array is hash-folded to 2^25 nibbles (16 MB), so it stays in the 126 MB
-//                 L2; folding can only add conflicts, never hide one.  Two flag sets alternate
+//                 The flag array is hash-folded to at most 2^25 nibbles (16 MB), so both sets stay in
+//                 the 50 MB L2 of an H100; folding can only add conflicts, never hide one.  Two flag sets alternate
 //                 between chunks: K1 of chunk k also zeroes the words chunk k-1 touched.
 //   K2 apply    : a request is SOLO when nothing else in the chunk can interact with it
 //                 (RA: WA clear; WA: R and W2 clear; WL: W2 clear).  Solo requests are applied
@@ -205,8 +205,8 @@ template <int KIND> struct Pre;
 template <int KIND> DINT_D Pre<KIND> prefetch(const Ctx& c, const uint8_t* rec, const KeyInfo& ki, const TypeInfo& ti);
 // Warp-wide variant used by k_apply: called by all 32 lanes (`active` = this lane has a request to fetch
 // for).  The KV kinds fetch table entries with several adjacent lanes per entry, so that an entry is ONE
-// 64-byte memory request instead of four 16-byte ones: random-access throughput on this chip is bounded
-// by outstanding requests per SM, not by bytes (tools/ubench.cu).
+// 64-byte memory request instead of four 16-byte ones: random-access throughput is bounded by outstanding
+// requests per SM, not by bytes (tools/ubench.cu measures it).
 template <int KIND>
 DINT_D Pre<KIND> prefetch_coop(const Ctx& c, const uint8_t* rec, const KeyInfo& ki, const TypeInfo& ti, bool active);
 
@@ -309,8 +309,8 @@ template <> DINT_D KeyInfo key_info<K_FASST>(const Ctx& c, const uint8_t* rec) {
   return k;
 }
 // The version of a lock_fasst slot: `ver` u32 per slot (144 MB at 36 M slots -- every READ costs one 64-byte HBM burst
-// for 4 bytes used).  A 16-bit hot array + cold high bits was measured (round 2, profiles/r02_variants.md): K2 -6 %,
-// step -2.4 %, and it degenerates to two accesses once a slot has seen 32768 commits (minutes of service): dropped.
+// for 4 bytes used).  A 16-bit hot array + cold high bits would degenerate to two accesses once a slot has seen 32768
+// commits (minutes of service).
 DINT_D uint32_t ver_load(const Ctx& c, uint32_t g) { return __ldcg(&c.ver[g]); }
 DINT_D void ver_store(const Ctx& c, uint32_t g, uint32_t v) { c.ver[g] = v; }
 template <> struct Pre<K_FASST> { uint32_t ver; };

@@ -58,10 +58,7 @@ template <int MSG> struct Stage {
 };
 
 // Persistent-CTA tile pipeline: CTA b owns tiles b, b + gridDim.x, ...; thread 0 keeps kStages - 1 TMA bulk loads in
-// flight ahead of the tile being processed.  (Dynamic assignment by a ticket counter was built and measured in round 2,
-// profiles/r02_variants.md: +17 % with the ticket drawn at the point of use, +5-7 % with the draw one iteration ahead,
-// and NO gain inside the multi-GPU step it was meant for -- 145.7 vs 144.5 us per batch at N = 2 -- because the kernels
-// of the step compete for the memory system, not for SM slots.  Dropped.)
+// flight ahead of the tile being processed.
 struct TileIter {
   uint32_t n_my;        // tiles owned by this CTA
   DINT_D uint32_t tile(uint32_t i) const { return blockIdx.x + i * gridDim.x; }
@@ -384,8 +381,6 @@ __global__ void __launch_bounds__(kThreads) k_log_scan(const Ctx c) {
 // ---------------------------------------------------------------------------------------------------
 // K2 apply
 // ---------------------------------------------------------------------------------------------------
-// (register caps were tried for the KV servers: 48 registers / 10 CTAs per SM measured 10 % slower than the
-// compiler's own 62 registers / 8 CTAs, and more registers / fewer CTAs slower still)
 template <int KIND, bool HAS_LOG>
 __global__ void __launch_bounds__(kTile) k_apply(const Ctx c) {
   using W = Wire<KIND>;

@@ -11,7 +11,6 @@
 //            shared memory into one run per shard, each run placed at the alignment of its destination so that it
 //            leaves with 16-byte stores.  Slots past a slab's total become padding records; the last CTA to finish
 //            raises the epoch flags of the peers (release, system scope) when the slabs live in peer memory.
-//            (Round 1 used two launches -- count, then scatter: 28 us per 2^20 records against about half that here.)
 //
 // The combine reads, per tile, one contiguous run per shard from the reply slabs and reassembles the tile in
 // request order; its only per-record state is the owner byte and, per tile, the first slot of each run.
@@ -315,7 +314,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_route_dispatch(const Ctx c, con
   }
   // ---- the last CTA to finish tells the peers that this source's slabs of epoch `epoch` are complete ----
   // (one system-scope fence per CTA, by the thread that counts the CTA as done, after the CTA barrier: cumulative over the
-  //  other threads' stores; a fence in every thread cost 4.4 stall cycles per issued instruction, profiles/r02_multigpu.md)
+  //  other threads' stores, instead of a fence in every thread)
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();

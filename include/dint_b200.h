@@ -1,5 +1,5 @@
 /*
- * dint_b200.h -- C ABI of libdint_b200.so, the B200-resident replacement for the per-request
+ * dint_b200.h -- C ABI of libdint_b200.so, the GPU-resident (H100) replacement for the per-request
  * server hot path of DINT (NSDI'24).
  *
  * The reference has no plugin/FFI API: the public interface of its hot path is the WIRE PROTOCOL

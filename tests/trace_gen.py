@@ -123,3 +123,16 @@ def tatp_random(n, n_subs, seed, oracle=None):
         rec["table"][i] = tb
         rec["key"][i] = key
     return wire.as_bytes(rec)
+
+
+# seeded traces whose replies from the unmodified reference server binaries are stored under
+# tests/golden/reference_replay/<name>.npz (tools/make_golden.py); (name, kind, trace)
+REFERENCE_REPLAY = [
+    ("fasst_random", wire.FASST, lambda: fasst_random(20000, 64, seed=11)),
+    ("lock2pl_random", wire.LOCK2PL, lambda: lock2pl_random(20000, 64, seed=12)),
+    ("log_random", wire.LOG, lambda: log_random(5000, seed=13)),
+    ("fasst_single_datagram", wire.FASST, lambda: fasst_random(1, 1, seed=14)),
+    ("fasst_one_slot", wire.FASST, lambda: fasst_random(6000, 1, seed=15)),                        # every request on ONE lock slot
+    ("lock2pl_release_wrap", wire.LOCK2PL, lambda: lock2pl_random(6000, 1, seed=16, p_release=0.7)),  # releases without a hold
+    ("lock2pl_full_u32_ids", wire.LOCK2PL, lambda: lock2pl_random(3000, 2**32 - 1, seed=17)),       # ids over the whole u32 range
+]

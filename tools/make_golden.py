@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz from the UNMODIFIED reference servers (oracle/_ref, built in place from
-/root/reference by `make -C oracle ref`).  Run in the build container only; the fixtures are committed.
+"""Generate tests/golden/*.npz from the UNMODIFIED reference servers (oracle/_ref, built in place from a
+reference checkout by `make -C oracle ref REF=<dir>`).  The fixtures are committed.
 
 Each fixture = {req: uint8[n*msg], resp: uint8[n*msg] as produced by `<server> 1` under the replay shim,
 kind, cfg: the oracle/engine configuration under which the same replies must come out}.  KV traces only
@@ -39,10 +39,22 @@ def closed_loop(kind, fam, clients, rounds, seed, **wl_kw):
     return req
 
 
+def save_replay():
+    """tests/golden/reference_replay/<name>.npz: the reference binary's replies to the traces of T.REFERENCE_REPLAY, stored
+    as reply XOR request (a reply rewrites a few fields of its request, so the difference compresses to almost nothing)."""
+    d = os.path.join(OUT, "reference_replay")
+    os.makedirs(d, exist_ok=True)
+    for name, kind, make in T.REFERENCE_REPLAY:
+        req = make()
+        ref, _ = O.run_ref(kind, req)
+        np.savez_compressed(os.path.join(d, name + ".npz"), resp_xor_req=ref ^ req)
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     O.build_oracle(ref=True)
-    assert O.ref_available(), "oracle/_ref is not built (is /root/reference mounted?)"
+    assert O.ref_available(), "oracle/_ref is not built (make -C oracle ref REF=<reference checkout>)"
+    save_replay()
     # lock_fasst
     save("fasst_ref_closed", wire.FASST, closed_loop(wire.FASST, REF, 256, 40, 20230), {})
     save("fasst_hot_closed", wire.FASST, closed_loop(wire.FASST, HOT, 256, 40, 20231), {})

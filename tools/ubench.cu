@@ -39,7 +39,8 @@ int main() {
   size_t bytes = 4ULL << 30;
   uint4* tbl; cudaMalloc(&tbl, bytes); cudaMemset(tbl, 1, bytes);
   uint32_t* out; cudaMalloc(&out, 4);
-  int sms = 148;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (size_t tb : {512ULL << 20, 4ULL << 30}) {
     run<4, 1>("64B ilp1 8cta", tbl, tb / 64, sms * 8, 256, 64, out);
     run<4, 2>("64B ilp2 8cta", tbl, tb / 64, sms * 8, 256, 32, out);
