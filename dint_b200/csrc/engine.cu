@@ -366,12 +366,18 @@ static int run_device(dint_engine* e, const uint8_t* req, uint64_t n, uint8_t* r
   return rc ? rc : kv_publish_counts(e, s);
 }
 
-static int pull_counters(dint_engine* e) {
-  unsigned long long h[4];
-  CU(cudaMemcpy(h, e->ctx.counters, sizeof h, cudaMemcpyDeviceToHost));
+static void stats_from_counters(dint_engine* e, const unsigned long long* h) {
   e->stats.errors = h[0];
   e->stats.conflicted = h[1];
   e->stats.max_run = h[2];
+  e->stats.ordered_fallbacks = h[3];
+  e->stats.bucket_split_tasks = h[4];
+  e->stats.writerless_chunks = h[5];
+}
+static int pull_counters(dint_engine* e) {
+  unsigned long long h[kNumCounters];
+  CU(cudaMemcpy(h, e->ctx.counters, sizeof h, cudaMemcpyDeviceToHost));
+  stats_from_counters(e, h);
   return DINT_OK;
 }
 
@@ -628,7 +634,7 @@ static int create_impl(dint_engine* e) {
   if ((rc = dalloc(e, &c.log_tilecnt, e->max_tiles))) return rc;
   if ((rc = dalloc(e, &c.log_tilebase, e->max_tiles))) return rc;
   if ((rc = dalloc(e, &c.log_total, 2))) return rc;
-  if ((rc = dalloc(e, &c.counters, 4))) return rc;
+  if ((rc = dalloc(e, &c.counters, kNumCounters))) return rc;
   if ((rc = dalloc(e, &c.gbar, 4))) return rc;
 
   switch (e->kind) {
@@ -914,8 +920,8 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
     if (rc) return rc;
     if (k >= 1 && (rc = copy_out_prev(k))) return rc;
   }
-  if (!e->h_counters) CU(cudaHostAlloc((void**)&e->h_counters, 4 * sizeof(unsigned long long), cudaHostAllocDefault));
-  CU(cudaMemcpyAsync(e->h_counters, e->ctx.counters, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
+  if (!e->h_counters) CU(cudaHostAlloc((void**)&e->h_counters, kNumCounters * sizeof(unsigned long long), cudaHostAllocDefault));
+  CU(cudaMemcpyAsync(e->h_counters, e->ctx.counters, kNumCounters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
   { int rc2 = kv_publish_counts(e, e->stream); if (rc2) return rc2; }
   const auto t_enq = std::chrono::steady_clock::now();
   CU(cudaStreamSynchronize(e->s_out));
@@ -928,9 +934,7 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
             std::chrono::duration<double, std::micro>(t_enq - t_begin).count(),
             std::chrono::duration<double, std::micro>(t_end - t_begin).count());
   }
-  e->stats.errors = e->h_counters[0];
-  e->stats.conflicted = e->h_counters[1];
-  e->stats.max_run = e->h_counters[2];
+  stats_from_counters(e, e->h_counters);
   return e->stats.errors != err_before ? DINT_EPROTO : DINT_OK;
 }
 
@@ -985,7 +989,9 @@ int dint_snapshot_restore(dint_snapshot* s, void* cuda_stream) {
     if (now[i].second != s->live[i].second) return set_err(DINT_EINVAL, "snapshot does not match the engine");
     CU(cudaMemcpyAsync(now[i].first, s->copy[i], now[i].second, cudaMemcpyDeviceToDevice, (cudaStream_t)cuda_stream));
   }
-  return DINT_OK;
+  // the KV tables' {live, used} counters went back too: refresh their host mirror, or the next call's kv_maintain
+  // would rehash a restored table on the occupancy it had before the restore
+  return kv_publish_counts(e, (cudaStream_t)cuda_stream);
 }
 void dint_snapshot_destroy(dint_snapshot* s) {
   if (!s) return;
@@ -1058,7 +1064,7 @@ void dint_reset_stats(dint_engine* e) {
   if (!e) return;
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
-  cudaMemset(e->ctx.counters, 0, 4 * sizeof(unsigned long long));
+  cudaMemset(e->ctx.counters, 0, kNumCounters * sizeof(unsigned long long));
   e->stats = dint_stats{};
   for (int i = 0; i < KT_NUM; i++) { e->kt_ms[i] = 0; e->kt_n[i] = 0; }
 }

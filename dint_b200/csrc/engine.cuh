@@ -44,6 +44,7 @@ constexpr int kMaxTables = 5;
 constexpr uint32_t kBucketCap = 128;    // ordered replay: bucket capacity (sorted in a warp's slice of shared memory)
 constexpr uint32_t kBucketFill = 64;    // K3: chunk / kBucketFill buckets (mean occupancy 64 if EVERY request were listed)
 constexpr int kStages = 3;              // TMA pipeline depth of the persistent K1/K2 CTAs
+constexpr int kNumCounters = 8;         // device counters (Ctx::counters), copied into dint_stats
 
 // what a request touches inside its group (conflict detection)
 enum : uint32_t { C_RA = 1, C_WA = 2, C_WL = 4 };
@@ -133,7 +134,8 @@ struct Ctx {
   unsigned long long* log_tilebase;  // [n_tiles] absolute append ordinal of the tile's first append (K1b)
   unsigned long long* log_total;     // [2]: [0] appends before this chunk ... running total, [1] this chunk's total
   // bookkeeping
-  unsigned long long* counters;   // [0] errors [1] conflicted [2] max_run
+  unsigned long long* counters;   // [kNumCounters]: [0] errors [1] conflicted [2] max_run [3] ordered_fallbacks
+                                  // [4] bucket_split_tasks [5] writerless_chunks (dint_stats)
   uint32_t* gbar;                 // k_ordered's grid barrier when it is not launched cooperatively
   uint32_t coop_launch;           // 1: k_ordered was launched cooperatively
   // where the replies go.  Default: `resp`, one contiguous array.  Inside the multi-GPU step the batch is W source

@@ -480,7 +480,10 @@ __global__ void __launch_bounds__(kTile) k_apply(const Ctx c) {
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
   }
-  if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (threadIdx.x == 0) {
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    if (blockIdx.x == 0 && !chunk_has_writer) atomicAdd(&c.counters[5], 1ULL);   // dint_stats.writerless_chunks
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -556,6 +559,7 @@ DINT_D void ordered_buckets(const Ctx& c, uint8_t* scratch) {
             for (uint32_t i = lane; i < ck; i += 32) wkeys[ek + i] = src[i];
           }
         } else {
+          if (pass == 0 && lane == 0) atomicAdd(&c.counters[4], 1ULL);                // dint_stats.bucket_split_tasks
           m = __shfl_sync(0xffffffffu, cnt, pass);
           const uint64_t* src = c.buckets + (size_t)(b0 + pass) * kBucketCap;
           for (uint32_t i = lane; i < m; i += 32) wkeys[i] = src[i];
@@ -694,6 +698,7 @@ __global__ void __launch_bounds__(kThreads) k_ordered(const Ctx c) {
   const uint32_t nc = c.nc_ord[0];
   const uint32_t overflow = c.nc_ord[1];
   if (nc == 0 || overflow == 0) return;               // the bucket path (inside the next K1) handles this chunk
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&c.counters[3], 1ULL);   // dint_stats.ordered_fallbacks
   GridBar grid{cg::this_grid(), c.gbar, c.coop_launch != 0};
   __shared__ uint64_t skeys[2048];                    // radix counters
   __shared__ uint32_t wsum[kThreads / 32];

@@ -90,7 +90,13 @@ typedef struct dint_stats {
   uint64_t h2d_bytes, d2h_bytes;
   uint64_t kv_rebuilds;     /* KV tables rehashed to reclaim tombstones (the reference frees entries on delete:
                                store/udp/kvs.h:124-133) */
-  uint64_t reserved[3];
+  /* which ordered-replay route the listed requests took (DESIGN.md section 3):
+     ordered_fallbacks:  chunks whose listed requests overflowed a bucket and were replayed by the radix-sort fallback
+     bucket_split_tasks: bucket-replay warp tasks that held more than a shared-memory slice and ran bucket by bucket
+     writerless_chunks:  chunks without a single writer, whose conflict check was skipped altogether */
+  uint64_t ordered_fallbacks;
+  uint64_t bucket_split_tasks;
+  uint64_t writerless_chunks;
 } dint_stats;
 
 /* Per-kernel device time, accumulated with CUDA events while profiling is on. */
