@@ -11,7 +11,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
-# DINT_LIB_TAG=<tag> (development only, tools/variants.sh): load / build libdint_b200_<tag>.so, compiled with DINT_NVCC_DEFINES
+# DINT_LIB_TAG=<tag> (development only): load libdint_b200_<tag>.so, or build it with DINT_NVCC_DEFINES when it is missing
 _TAG = os.environ.get("DINT_LIB_TAG", "")
 LIB = os.path.join(LIBDIR, f"libdint_b200_{_TAG}.so" if _TAG else "libdint_b200.so")
 WL_LIB = os.path.join(LIBDIR, "libdint_wl.so")
@@ -48,7 +48,8 @@ def build(force=False, verbose=False):
         return LIB                    # a read-only tree: use the libraries it was built with
     os.makedirs(LIBDIR, exist_ok=True)
     cu_src = _sources((".cu", ".cuh", ".h"))
-    if force or _newer(LIB, cu_src):
+    # a tagged library that exists is used as built: it may be a frozen build of another commit for an A/B run
+    if (force or _newer(LIB, cu_src)) and not (_TAG and os.path.exists(LIB)):
         nvcc = find_nvcc()
         if nvcc is None:
             raise RuntimeError("nvcc not found: cannot build libdint_b200.so (there is no CPU fallback)")

@@ -256,6 +256,8 @@ static void fill_chunk_ctx(dint_engine* e, Ctx& c) {
   c.flags = e->d_flags[cur];
   c.flags_prev = e->d_flags[cur ^ 1];
   c.prev_n = e->prev_n;
+  // whole-set clear once there is at least one request per 128-byte line of the set (2^20-request chunks: 8 per line)
+  c.clear_set = (uint64_t)(c.flags_mask + 1) / 256 <= e->prev_n ? 1u : 0u;
   c.nc_cur = e->d_nc + 4 * cur;          // {listed, overflow, a writer exists, -}
   c.nc_ord = e->d_nc + 4 * (cur ^ 1);
   c.ord_pending = e->ord_pending ? 1u : 0u;

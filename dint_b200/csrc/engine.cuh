@@ -12,7 +12,8 @@
 //                 nibble holds R (an RA exists), WA, WL and W2 (two or more writers of one class).
 //                 The flag array is hash-folded to at most 2^25 nibbles (16 MB), so both sets stay in
 //                 the 50 MB L2 of an H100; folding can only add conflicts, never hide one.  Two flag sets alternate
-//                 between chunks: K1 of chunk k also zeroes the words chunk k-1 touched.
+//                 between chunks: K1 of chunk k also zeroes the words chunk k-1 touched (for a large chunk, the
+//                 whole set, with coalesced stores).
 //   K2 apply    : a request is SOLO when nothing else in the chunk can interact with it
 //                 (RA: WA clear; WA: R and W2 clear; WL: W2 clear).  Solo requests are applied
 //                 directly, one thread each, against the HBM-resident state and their tile is
@@ -97,6 +98,7 @@ struct Ctx {
   uint32_t* grp;           // [chunk] group id per request of THIS chunk (0xffffffff: none)
   const uint32_t* grp_prev;  // [prev_n] group ids of the previous chunk (its flags are cleared by this K1)
   uint32_t prev_n;
+  uint32_t clear_set;      // 1: K1 zeroes the previous chunk's whole flag set instead of the words its prev_n requests set
   uint32_t* flags;         // this chunk's flag set: 2^flags_log2 nibbles
   uint32_t* flags_prev;    // the previous chunk's flag set
   uint32_t flags_mask;     // 2^flags_log2 - 1

@@ -270,10 +270,18 @@ __global__ void __launch_bounds__(kTile) k_classify(const Ctx c) {
   if (threadIdx.x == 0)
     for (uint32_t i = 0; i < NS && i < it.n_my; i++) issue_tile_load<W::MSG>(c, smem, full, it, i);
 
-  // retire the previous chunk's flags: every word it touched is zeroed (all of that set's nibbles
-  // were written by that chunk, so whole-word stores are exact).  Loads are batched four deep so that
-  // the kernel start pays one memory latency, not one per element.
-  for (uint32_t i = blockIdx.x * kTile + threadIdx.x; i < c.prev_n; i += 4 * gridDim.x * kTile) {
+  // retire the previous chunk's flags.  A large chunk touches most 128-byte lines of its set, so the whole set is
+  // zeroed with coalesced 16-byte stores (the rest of it is zero already): a few full-line writes per line instead
+  // of one random 4-byte store per request, and no group-id loads.
+  if (c.clear_set) {
+    uint4* f4 = (uint4*)c.flags_prev;
+    const uint32_t n4 = (c.flags_mask + 1) / 32;           // nibbles / 8 per word / 4 words per uint4
+    for (uint32_t i = blockIdx.x * kTile + threadIdx.x; i < n4; i += gridDim.x * kTile) f4[i] = make_uint4(0, 0, 0, 0);
+  }
+  // Otherwise every word the previous chunk touched is zeroed (all of that set's nibbles were written by that chunk,
+  // so whole-word stores are exact).  Loads are batched four deep so that the kernel start pays one memory latency,
+  // not one per element.
+  for (uint32_t i = blockIdx.x * kTile + threadIdx.x; !c.clear_set && i < c.prev_n; i += 4 * gridDim.x * kTile) {
     uint32_t g[4];
 #pragma unroll
     for (int u = 0; u < 4; u++) {

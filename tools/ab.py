@@ -10,6 +10,10 @@ from gpu_probe import probe
 n = 1 << 22
 tag = " ".join(f"{k}={v}" for k, v in os.environ.items() if k.startswith("DINT_"))
 print("==", tag or "defaults")
+# the card, its power limit and its SM clocks belong beside every time below
+import subprocess
+print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                     capture_output=True, text=True).stdout.strip())
 probe(wire.FASST, T.fasst_random(n, 24_000_000, seed=1, weights=(0.6, 0.15, 0.05, 0.2)), chunk=int(os.environ.get("CHUNK", 1 << 20)))
 if "--store" in sys.argv:
     probe(wire.STORE, T.store_random(n, 2_000_000, seed=4, p_set=0.0, p_miss=0.0), chunk=1 << 20, populate=True)
