@@ -8,6 +8,7 @@
 #include <cstring>
 #include <string>
 #include <chrono>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/dint_b200.h"
@@ -35,6 +36,30 @@ static int set_err(int code, const char* what, cudaError_t ce = cudaSuccess) {
 static const uint32_t kMsgSize[DINT_NUM_KINDS] = {6, 9, 53, 53, 55, 23};
 static const uint32_t kLogEntry[DINT_NUM_KINDS] = {0, 0, 56, 0, 64, 32};
 static const uint32_t kValSize[DINT_NUM_KINDS] = {0, 0, 0, 40, 40, 8};
+
+// The one place where an engine's run-time kind picks the kernel templates: calls f(std::integral_constant<int, K>{})
+// and returns what f returns.  Record-size-keyed kernels are instantiated with Wire<K>::MSG.
+template <class F>
+static int with_kind(int kind, F&& f) {
+  switch (kind) {
+    case DINT_LOCK2PL: return f(std::integral_constant<int, K_LOCK2PL>{});
+    case DINT_FASST: return f(std::integral_constant<int, K_FASST>{});
+    case DINT_LOG: return f(std::integral_constant<int, K_LOG>{});
+    case DINT_STORE: return f(std::integral_constant<int, K_STORE>{});
+    case DINT_TATP: return f(std::integral_constant<int, K_TATP>{});
+    case DINT_SMALLBANK: return f(std::integral_constant<int, K_SMALLBANK>{});
+  }
+  return set_err(DINT_EINVAL, "bad kind");
+}
+
+// Where the replies of one run_device call go when they are not one contiguous array: inside the multi-GPU step the
+// batch is W source slabs of seg_tiles tiles each, and the replies of slab s go straight into source s's return buffer.
+struct StepTarget {
+  uint32_t seg_tiles;                 // tiles per source slab
+  uint64_t seg_resp[kMaxShards];      // reply slab of source s (device address, possibly peer memory)
+  bool pad_ok;                        // type 0xFE records are slab padding (else: invalid)
+  const uint32_t* skip;               // non-zero: a slab overflowed, serve nothing more (see k_p2p_wait)
+};
 
 enum { KT_CLASSIFY = 0, KT_LOGSCAN, KT_APPLY, KT_ORDERED, KT_LOAD, KT_NUM };
 static const char* kKernelNames[KT_NUM] = {"k_classify", "k_log_scan", "k_apply", "k_ordered", "k_kv_load"};
@@ -76,11 +101,6 @@ struct dint_engine {
   uint8_t* ord_resp = nullptr;               //   ... and live in this reply array
   const uint8_t* ord_req = nullptr;          //   ... their request bytes in this one
   uint32_t ord_tile0 = 0;                    //   ... which starts at this tile of its batch
-  // segmented replies (multi-GPU step): set around run_device by the sharded step, zero otherwise
-  uint32_t seg_tiles = 0;
-  uint64_t seg_resp[kMaxShards]{};
-  bool pad_ok = false;
-  const uint32_t* skip = nullptr;
   uint32_t smem_classify = 0;                // K1: max(stages, ordered-replay slices)
   uint32_t* d_nc = nullptr;                  // [2 chunks][2]: listed / overflow counters
   uint32_t* d_route = nullptr;               // multi-GPU dispatch scratch (per-tile per-shard counts)
@@ -171,7 +191,7 @@ static cudaError_t launch_ex(dint_engine* e, void (*kern)(Args...), int grid, in
 // One chunk: K1 (classify this chunk + replay the previous chunk's listed requests), K2 (apply), and the
 // fallback launch that only does work when one of THIS chunk's buckets overflowed.  c.n == 0 = flush: K1
 // alone, replaying the last chunk's listed requests.
-template <int KIND, bool HAS_LOG>
+template <int KIND>
 static int launch_chunk_t(dint_engine* e, const Ctx& c, cudaStream_t s) {
   {
     ProfScope ps(e, s, KT_CLASSIFY);
@@ -179,17 +199,17 @@ static int launch_chunk_t(dint_engine* e, const Ctx& c, cudaStream_t s) {
     if (clr > want) want = clr;
     int grid = (want < e->grid_classify && !c.ord_pending) ? want : e->grid_classify;
     if (c.n == 0 && e->sms > 0 && grid > 8 * e->sms) grid = 8 * e->sms;     // a flush launch only replays: 32 warps per SM are plenty
-    CU(launch_ex(e, k_classify<KIND, HAS_LOG>, grid, kTile, e->smem_classify, s, false, c));
+    CU(launch_ex(e, k_classify<KIND>, grid, kTile, e->smem_classify, s, false, c));
   }
   if (c.n == 0) { CU(cudaGetLastError()); return DINT_OK; }
-  if (HAS_LOG) {
+  if (kHasLog<KIND>) {
     ProfScope ps(e, s, KT_LOGSCAN);
     k_log_scan<<<1, kThreads, 0, s>>>(c);
   }
   {
     ProfScope ps(e, s, KT_APPLY);
     int grid = (int)c.n_tiles < e->grid_apply ? (int)c.n_tiles : e->grid_apply;
-    CU(launch_ex(e, k_apply<KIND, HAS_LOG>, grid, kTile, e->smem_stage, s, false, c));
+    CU(launch_ex(e, k_apply<KIND>, grid, kTile, e->smem_stage, s, false, c));
   }
   if (KIND != K_LOG) {   // the log server has no per-key state: nothing to order
     ProfScope ps(e, s, KT_ORDERED);
@@ -211,18 +231,10 @@ static int launch_chunk_t(dint_engine* e, const Ctx& c, cudaStream_t s) {
 }
 
 static int launch_chunk(dint_engine* e, const Ctx& c, cudaStream_t s) {
-  switch (e->kind) {
-    case DINT_LOCK2PL: return launch_chunk_t<K_LOCK2PL, false>(e, c, s);
-    case DINT_FASST: return launch_chunk_t<K_FASST, false>(e, c, s);
-    case DINT_LOG: return launch_chunk_t<K_LOG, true>(e, c, s);
-    case DINT_STORE: return launch_chunk_t<K_STORE, false>(e, c, s);
-    case DINT_TATP: return launch_chunk_t<K_TATP, true>(e, c, s);
-    case DINT_SMALLBANK: return launch_chunk_t<K_SMALLBANK, true>(e, c, s);
-  }
-  return DINT_EINVAL;
+  return with_kind(e->kind, [&](auto k) { return launch_chunk_t<decltype(k)::value>(e, c, s); });
 }
 
-template <int KIND, bool HAS_LOG>
+template <int KIND>
 static int grids_for(dint_engine* e) {
   int per_sm = 0, sms = 0;
   CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device));
@@ -230,15 +242,15 @@ static int grids_for(dint_engine* e) {
   e->grid_route = 4 * sms;
   e->smem_stage = Stage<Wire<KIND>::MSG>::N * Stage<Wire<KIND>::MSG>::BYTES;
   if (e->smem_stage > 48 * 1024) {
-    CU(cudaFuncSetAttribute(k_classify<KIND, HAS_LOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_stage));
-    CU(cudaFuncSetAttribute(k_apply<KIND, HAS_LOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_stage));
+    CU(cudaFuncSetAttribute(k_classify<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_stage));
+    CU(cudaFuncSetAttribute(k_apply<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->smem_stage));
   }
   e->smem_classify = e->smem_stage;
   if (KIND != K_LOG && (kTile / 32) * OrdSlice<KIND>::BYTES > e->smem_classify) e->smem_classify = (kTile / 32) * OrdSlice<KIND>::BYTES;
-  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify<KIND, HAS_LOG>, kTile, e->smem_classify));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify<KIND>, kTile, e->smem_classify));
   if (per_sm < 1) return set_err(DINT_EIO, "k_classify cannot be resident");
   e->grid_classify = per_sm * sms;
-  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply<KIND, HAS_LOG>, kTile, e->smem_stage));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_apply<KIND>, kTile, e->smem_stage));
   if (per_sm < 1) return set_err(DINT_EIO, "k_apply cannot be resident");
   e->grid_apply = per_sm * sms;
   if (KIND == K_LOG) { e->coop_grid = 1; return DINT_OK; }
@@ -249,7 +261,7 @@ static int grids_for(dint_engine* e) {
   return DINT_OK;
 }
 
-static void fill_chunk_ctx(dint_engine* e, Ctx& c) {
+static void fill_chunk_ctx(dint_engine* e, Ctx& c, const StepTarget* tgt) {
   const int cur = (int)(e->chunk_seq & 1);
   c.grp = e->d_grp[cur];
   c.grp_prev = e->d_grp[cur ^ 1];
@@ -264,21 +276,24 @@ static void fill_chunk_ctx(dint_engine* e, Ctx& c) {
   c.ord_resp = e->ord_resp;
   c.ord_req = e->ord_req;
   c.ord_tile0 = e->ord_tile0;
-  c.seg_tiles = e->seg_tiles;
-  c.pad_ok = e->pad_ok ? 1u : 0u;
-  c.skip = e->skip;
-  for (int i = 0; i < kMaxShards; i++) c.seg_resp[i] = e->seg_resp[i];
+  if (tgt) {                             // else e->ctx's zeros: contiguous replies in c.resp, no padding, no skip word
+    c.seg_tiles = tgt->seg_tiles;
+    c.pad_ok = tgt->pad_ok ? 1u : 0u;
+    c.skip = tgt->skip;
+    for (int i = 0; i < kMaxShards; i++) c.seg_resp[i] = tgt->seg_resp[i];
+  }
 }
 
 // one chunk (n <= e->chunk); leaves its listed requests pending until the next chunk or flush_ordered()
-static int submit_chunk(dint_engine* e, const uint8_t* req, uint32_t n, uint8_t* resp, cudaStream_t s, uint32_t tile0 = 0) {
+static int submit_chunk(dint_engine* e, const uint8_t* req, uint32_t n, uint8_t* resp, cudaStream_t s, uint32_t tile0 = 0,
+                        const StepTarget* tgt = nullptr) {
   Ctx c = e->ctx;
   c.n = n;
   c.n_tiles = (n + kTile - 1) / kTile;
   c.req = req;
   c.resp = resp;
   c.tile0 = tile0;
-  fill_chunk_ctx(e, c);
+  fill_chunk_ctx(e, c, tgt);
   int rc = launch_chunk(e, c, s);
   if (rc) return rc;
   e->chunk_seq++;
@@ -293,14 +308,14 @@ static int submit_chunk(dint_engine* e, const uint8_t* req, uint32_t n, uint8_t*
 }
 
 // replays the last chunk's listed requests (and retires its flags); after this every reply is final
-static int flush_ordered(dint_engine* e, cudaStream_t s) {
+static int flush_ordered(dint_engine* e, cudaStream_t s, const StepTarget* tgt = nullptr) {
   if (!e->ord_pending) return DINT_OK;
   Ctx c = e->ctx;
   c.n = 0;
   c.n_tiles = 0;
   c.req = nullptr;
   c.resp = nullptr;
-  fill_chunk_ctx(e, c);
+  fill_chunk_ctx(e, c, tgt);
   c.prev_n = 0;                  // replay only: that chunk's flags are retired by the NEXT chunk's K1 as usual (next to its tile
                                  // loads), not by this launch, which a caller is waiting for
   int rc = launch_chunk(e, c, s);
@@ -337,8 +352,11 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
     N.entries = (uint8_t*)fresh;
     {
       ProfScope ps(e, s, KT_LOAD);
-      if (e->kind == DINT_SMALLBANK) k_kv_rehash<8><<<e->sms * 8, 256, 0, s>>>(T, N);
-      else k_kv_rehash<40><<<e->sms * 8, 256, 0, s>>>(T, N);
+      with_kind(e->kind, [&](auto k) {
+        constexpr int K = decltype(k)::value;
+        if constexpr (K == K_STORE || K == K_TATP || K == K_SMALLBANK) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
+        return DINT_OK;
+      });
     }
     CU(cudaStreamSynchronize(s));
     for (auto& p : e->allocs) if (p == (void*)T.entries) p = fresh;
@@ -357,14 +375,18 @@ static int kv_publish_counts(dint_engine* e, cudaStream_t s) {
   return DINT_OK;
 }
 
-static int run_device(dint_engine* e, const uint8_t* req, uint64_t n, uint8_t* resp, cudaStream_t s) {
+// One call of n requests on stream s.  The replies go to `resp`, or, with a target, where `tgt` says (the multi-GPU
+// step; resp is then null).  The target belongs to this call alone: K1 of a chunk also replays the previous chunk's
+// listed requests under the CURRENT chunk's target, and that is right only because every call ends in flush_ordered,
+// so no chunk of this call is left to be replayed by the next call under another target.  Keep it that way.
+static int run_device(dint_engine* e, const uint8_t* req, uint64_t n, uint8_t* resp, cudaStream_t s, const StepTarget* tgt = nullptr) {
   { int rc = kv_maintain(e, s); if (rc) return rc; }
   for (uint64_t off = 0; off < n; off += e->chunk) {
     uint32_t cn = (uint32_t)((n - off < e->chunk) ? (n - off) : e->chunk);
-    int rc = submit_chunk(e, req + off * e->msg, cn, resp ? resp + off * e->msg : nullptr, s, (uint32_t)(off / kTile));
+    int rc = submit_chunk(e, req + off * e->msg, cn, resp ? resp + off * e->msg : nullptr, s, (uint32_t)(off / kTile), tgt);
     if (rc) return rc;
   }
-  int rc = flush_ordered(e, s);
+  int rc = flush_ordered(e, s, tgt);
   return rc ? rc : kv_publish_counts(e, s);
 }
 
@@ -381,16 +403,6 @@ static int pull_counters(dint_engine* e) {
   CU(cudaMemcpy(h, e->ctx.counters, sizeof h, cudaMemcpyDeviceToHost));
   stats_from_counters(e, h);
   return DINT_OK;
-}
-
-template <int MSG>
-static void route_scatter_t(const uint8_t* rq, const uint8_t* ow, uint32_t n, uint32_t world, const uint32_t* tb,
-                            const uint32_t* totals, uint8_t* out, uint32_t* perm, uint32_t tiles, cudaStream_t s) {
-  k_exact_scatter<MSG><<<tiles, kThreads, 0, s>>>(rq, ow, n, world, tb, totals, out, perm);
-}
-template <int MSG>
-static void route_unpermute_t(const uint8_t* sorted, const uint32_t* perm, uint32_t n, uint8_t* out, cudaStream_t s) {
-  k_exact_unpermute<MSG><<<(n + kThreads - 1) / kThreads, kThreads, 0, s>>>(sorted, perm, n, out);
 }
 
 // Host-path slice sizes for a call of n requests (see dint_submit): slices double from `mn` up to the plateau
@@ -639,15 +651,7 @@ static int create_impl(dint_engine* e) {
   if ((rc = dalloc(e, &c.counters, kNumCounters))) return rc;
   if ((rc = dalloc(e, &c.gbar, 4))) return rc;
 
-  switch (e->kind) {
-    case DINT_LOCK2PL: rc = grids_for<K_LOCK2PL, false>(e); break;
-    case DINT_FASST: rc = grids_for<K_FASST, false>(e); break;
-    case DINT_LOG: rc = grids_for<K_LOG, true>(e); break;
-    case DINT_STORE: rc = grids_for<K_STORE, false>(e); break;
-    case DINT_TATP: rc = grids_for<K_TATP, true>(e); break;
-    default: rc = grids_for<K_SMALLBANK, true>(e); break;
-  }
-  if (rc) return rc;
+  if ((rc = with_kind(e->kind, [&](auto k) { return grids_for<decltype(k)::value>(e); }))) return rc;
   int coop = 0;
   CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, e->device));
   if (!coop) return set_err(DINT_ENODEV, "device lacks cooperative launch");
@@ -697,14 +701,10 @@ int dint_route_owner(dint_engine* e, const void* req_dev, uint64_t n, uint8_t* o
   const uint32_t blocks = (uint32_t)((n + kThreads - 1) / kThreads);
   const uint8_t* rq = (const uint8_t*)req_dev;
   e->stats.kernel_launches++;
-  switch (e->kind) {
-    case DINT_LOCK2PL: k_route_owner<K_LOCK2PL><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-    case DINT_FASST: k_route_owner<K_FASST><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-    case DINT_LOG: k_route_owner<K_LOG><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-    case DINT_STORE: k_route_owner<K_STORE><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-    case DINT_TATP: k_route_owner<K_TATP><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-    default: k_route_owner<K_SMALLBANK><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev); break;
-  }
+  with_kind(e->kind, [&](auto k) {
+    k_route_owner<decltype(k)::value><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev);
+    return DINT_OK;
+  });
   CU(cudaGetLastError());
   return DINT_OK;
 }
@@ -728,13 +728,10 @@ int dint_route_partition(dint_engine* e, const void* req_dev, const uint8_t* own
   k_exact_scan<<<n_shards, kThreads, 0, s>>>(tilecnt, tiles, totals);
   const uint8_t* rq = (const uint8_t*)req_dev;
   uint8_t* out = (uint8_t*)sorted_dev;
-  switch (e->msg) {
-    case 6: route_scatter_t<6>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev, tiles, s); break;
-    case 9: route_scatter_t<9>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev, tiles, s); break;
-    case 23: route_scatter_t<23>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev, tiles, s); break;
-    case 53: route_scatter_t<53>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev, tiles, s); break;
-    default: route_scatter_t<55>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev, tiles, s); break;
-  }
+  with_kind(e->kind, [&](auto k) {
+    k_exact_scatter<Wire<decltype(k)::value>::MSG><<<tiles, kThreads, 0, s>>>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev);
+    return DINT_OK;
+  });
   CU(cudaMemcpyAsync(counts_dev, totals, n_shards * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   CU(cudaGetLastError());
   return DINT_OK;
@@ -766,14 +763,7 @@ int dint_route_dispatch(dint_engine* e, const void* req_dev, const uint8_t* owne
   for (uint32_t i = 0; i < kMaxShards; i++) { a.slab.p[i] = slab_ptrs->p[i]; a.sig.p[i] = sig_ptrs ? sig_ptrs->p[i] : 0; }
   cudaStream_t s = (cudaStream_t)cuda_stream;
   e->stats.kernel_launches += 1;
-  switch (e->kind) {
-    case DINT_LOCK2PL: return route_dispatch_t<K_LOCK2PL>(e, a, s);
-    case DINT_FASST: return route_dispatch_t<K_FASST>(e, a, s);
-    case DINT_LOG: return route_dispatch_t<K_LOG>(e, a, s);
-    case DINT_STORE: return route_dispatch_t<K_STORE>(e, a, s);
-    case DINT_TATP: return route_dispatch_t<K_TATP>(e, a, s);
-    default: return route_dispatch_t<K_SMALLBANK>(e, a, s);
-  }
+  return with_kind(e->kind, [&](auto k) { return route_dispatch_t<decltype(k)::value>(e, a, s); });
 }
 
 int dint_route_combine(dint_engine* e, const dint_peer_ptrs* reply_slab_ptrs, const uint8_t* owner_dev, const uint32_t* tilebase_dev,
@@ -795,13 +785,7 @@ int dint_route_combine(dint_engine* e, const dint_peer_ptrs* reply_slab_ptrs, co
   for (uint32_t i = 0; i < kMaxShards; i++) a.slab.p[i] = reply_slab_ptrs->p[i];
   cudaStream_t s = (cudaStream_t)cuda_stream;
   e->stats.kernel_launches++;
-  switch (e->msg) {
-    case 6: return route_combine_t<6>(e, a, s);
-    case 9: return route_combine_t<9>(e, a, s);
-    case 23: return route_combine_t<23>(e, a, s);
-    case 53: return route_combine_t<53>(e, a, s);
-    default: return route_combine_t<55>(e, a, s);
-  }
+  return with_kind(e->kind, [&](auto k) { return route_combine_t<Wire<decltype(k)::value>::MSG>(e, a, s); });
 }
 
 int dint_p2p_wait(dint_engine* e, const uint32_t* local_sig_dev, uint32_t n_shards, uint32_t epoch, uint32_t* flags_dev, void* cuda_stream) {
@@ -832,13 +816,10 @@ int dint_route_unpermute(dint_engine* e, const void* sorted_dev, const uint32_t*
   e->stats.kernel_launches++;
   const uint8_t* in = (const uint8_t*)sorted_dev;
   uint8_t* out = (uint8_t*)out_dev;
-  switch (e->msg) {
-    case 6: route_unpermute_t<6>(in, perm_dev, (uint32_t)n, out, s); break;
-    case 9: route_unpermute_t<9>(in, perm_dev, (uint32_t)n, out, s); break;
-    case 23: route_unpermute_t<23>(in, perm_dev, (uint32_t)n, out, s); break;
-    case 53: route_unpermute_t<53>(in, perm_dev, (uint32_t)n, out, s); break;
-    default: route_unpermute_t<55>(in, perm_dev, (uint32_t)n, out, s); break;
-  }
+  with_kind(e->kind, [&](auto k) {
+    k_exact_unpermute<Wire<decltype(k)::value>::MSG><<<(uint32_t)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>(in, perm_dev, (uint32_t)n, out);
+    return DINT_OK;
+  });
   CU(cudaGetLastError());
   return DINT_OK;
 }
@@ -1274,14 +1255,9 @@ static int shard_engine(dint_shard_ctx* c, uint32_t slot, uint32_t ep, uint32_t 
   const size_t slab = (size_t)cap * e->msg;
   k_p2p_wait<<<1, 32, 0, st>>>(c->my_req + s * 8, c->W, ep, c->flags + 1, c->flags + 2);     // every source's slab has arrived (or one did not fit)
   shard_mark(c, slot, 2, st);
-  e->seg_tiles = cap / kTile;
-  e->pad_ok = true;
-  e->skip = c->flags + 2;
-  for (uint32_t r = 0; r < c->W; r++) e->seg_resp[r] = c->retbox[s][r] + (uint64_t)c->me * slab;   // my slab inside source r's return buffer
-  int rc = run_device(e, (const uint8_t*)c->inbox[s][c->me], (uint64_t)c->W * cap, nullptr, st);
-  e->seg_tiles = 0;
-  e->pad_ok = false;
-  e->skip = nullptr;
+  StepTarget tgt{cap / kTile, {}, true, c->flags + 2};
+  for (uint32_t r = 0; r < c->W; r++) tgt.seg_resp[r] = c->retbox[s][r] + (uint64_t)c->me * slab;   // my slab inside source r's return buffer
+  int rc = run_device(e, (const uint8_t*)c->inbox[s][c->me], (uint64_t)c->W * cap, nullptr, st, &tgt);
   if (rc) return rc;
   k_p2p_signal<<<1, 32, 0, st>>>(c->sigrsp, c->W, c->me, ep);
   shard_mark(c, slot, 3, st);

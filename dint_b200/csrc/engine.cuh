@@ -37,6 +37,8 @@
 namespace dint {
 
 enum Kind { K_LOCK2PL = 0, K_FASST = 1, K_LOG = 2, K_STORE = 3, K_TATP = 4, K_SMALLBANK = 5 };
+// the kinds whose requests append to a commit log (K1 counts the appends per tile, K1b turns them into ring ordinals)
+template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK;
 
 constexpr int kTile = 128;       // wire records per tile = threads per CTA in K1/K2 (16 CTAs, i.e. 16 independent
                                  // latency chains, per SM)

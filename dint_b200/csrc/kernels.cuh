@@ -48,6 +48,40 @@ DINT_D void tile_rank2(bool a, bool b, uint32_t* scratch, uint32_t& ra, uint32_t
   tb = tot >> 16;
 }
 
+// Exclusive scan of n counts by one CTA of kThreads threads: out[i] = start + in[0] + ... + in[i-1], in slices of
+// kThreads with the running carry in shared memory.  Returns start + the sum of all n counts.  `start` is taken from
+// thread 0; `wsum` is kThreads/32 words of shared memory.  in == out is allowed (every element is read and written by
+// the same thread).  Contains __syncthreads(): every thread of the CTA calls it.
+template <class T>
+DINT_D T cta_exclusive_scan(const uint32_t* in, T* out, uint32_t n, T start, uint32_t* wsum) {
+  __shared__ T carry;
+  if (threadIdx.x == 0) carry = start;
+  __syncthreads();
+  for (uint32_t base = 0; base < n; base += kThreads) {
+    const uint32_t i = base + threadIdx.x;
+    const uint32_t v = i < n ? in[i] : 0;
+    uint32_t x = v;                       // inclusive warp scan
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+      if ((int)lane_id() >= o) x += y;
+    }
+    if (lane_id() == 31) wsum[warp_id()] = x;
+    __syncthreads();
+    uint32_t woff = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; w++) {
+      if (w < (int)warp_id()) woff += wsum[w];
+      tot += wsum[w];
+    }
+    if (i < n) out[i] = carry + woff + (x - v);
+    __syncthreads();
+    if (threadIdx.x == 0) carry += tot;
+    __syncthreads();
+  }
+  return carry;
+}
+
 DINT_D uint32_t bucket_of(uint32_t g, uint32_t log2p) { return log2p ? (g * 0x9E3779B1u) >> (32 - log2p) : 0; }
 
 // bytes of one pipeline stage: a tile of wire records, padded so every stage stays 128-byte aligned
@@ -119,8 +153,8 @@ __global__ void __launch_bounds__(kThreads) k_route_owner(const Ctx c, const uin
 }
 
 // ---- multi-GPU dispatch: stable partition of a batch by owner shard -------------------------------------
-// (1) k_route_count: per 256-record tile, how many records go to each shard;  (2) k_exact_scan (one CTA):
-// exclusive offsets -- shard-major, then tile order -- and the per-shard totals;  (3) k_route_scatter: every
+// (1) k_exact_count: per 256-record tile, how many records go to each shard;  (2) k_exact_scan (one CTA per shard):
+// exclusive offsets -- shard-major, then tile order -- and the per-shard totals;  (3) k_exact_scatter: every
 // record is copied to its slot (stable inside a shard: tile order, then thread order) and the inverse
 // permutation is recorded.  Afterwards the wire records sit grouped by destination, ready for the exchange.
 constexpr int kMaxShards = 8;
@@ -138,33 +172,9 @@ __global__ void __launch_bounds__(kThreads) k_exact_count(const uint8_t* owner, 
 __global__ void __launch_bounds__(kThreads) k_exact_scan(uint32_t* tilecnt, uint32_t n_tiles, uint32_t* totals) {
   // one CTA per shard: exclusive scan of that shard's row of per-tile counts, row total -> totals[shard]
   __shared__ uint32_t wsum[kThreads / 32];
-  __shared__ uint32_t carry;
   uint32_t* row = tilecnt + (size_t)blockIdx.x * n_tiles;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (uint32_t base = 0; base < n_tiles; base += kThreads) {
-    const uint32_t i = base + threadIdx.x;
-    const uint32_t v = i < n_tiles ? row[i] : 0;
-    uint32_t x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-      if ((int)lane_id() >= o) x += y;
-    }
-    if (lane_id() == 31) wsum[warp_id()] = x;
-    __syncthreads();
-    uint32_t woff = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; w++) {
-      if (w < (int)warp_id()) woff += wsum[w];
-      tot += wsum[w];
-    }
-    if (i < n_tiles) row[i] = carry + woff + (x - v);
-    __syncthreads();
-    if (threadIdx.x == 0) carry += tot;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) totals[blockIdx.x] = carry;
+  const uint32_t total = cta_exclusive_scan<uint32_t>(row, row, n_tiles, 0u, wsum);
+  if (threadIdx.x == 0) totals[blockIdx.x] = total;
 }
 template <int MSG>
 __global__ void __launch_bounds__(kThreads) k_exact_scatter(const uint8_t* req, const uint8_t* owner, uint32_t n, uint32_t world,
@@ -242,7 +252,7 @@ template <int KIND> DINT_D void ordered_buckets(const Ctx& c, uint8_t* scratch);
 // ---------------------------------------------------------------------------------------------------
 // K1 classify (+ clears the flag words of the previous chunk)
 // ---------------------------------------------------------------------------------------------------
-template <int KIND, bool HAS_LOG>
+template <int KIND>
 __global__ void __launch_bounds__(kTile) k_classify(const Ctx c) {
   using W = Wire<KIND>;
   constexpr uint32_t NS = Stage<W::MSG>::N;
@@ -334,7 +344,7 @@ __global__ void __launch_bounds__(kTile) k_classify(const Ctx c) {
     }
     if (pend_w && ((pend_old >> pend_sh) & pend_test)) atomicOr(pend_w, F_W2 << pend_sh);
     pend_old = new_old; pend_test = new_test; pend_sh = new_sh; pend_w = new_w;
-    if (HAS_LOG) {
+    if (kHasLog<KIND>) {
       uint32_t total;
       (void)tile_rank(is_log, scratch, total);          // contains the CTA barriers that free the stage
       if (threadIdx.x == 0) c.log_tilecnt[it.tile(i)] = total;
@@ -354,42 +364,19 @@ __global__ void __launch_bounds__(kTile) k_classify(const Ctx c) {
 // K1b: absolute append ordinal of every tile's first log append (single CTA).
 __global__ void __launch_bounds__(kThreads) k_log_scan(const Ctx c) {
   if (c.skip && __ldcg(c.skip)) return;
-  __shared__ unsigned long long carry;
   __shared__ uint32_t wsum[kThreads / 32];
-  if (threadIdx.x == 0) carry = c.log_total[0];
-  __syncthreads();
-  for (uint32_t base = 0; base < c.n_tiles; base += kThreads) {
-    uint32_t i = base + threadIdx.x;
-    uint32_t v = i < c.n_tiles ? c.log_tilecnt[i] : 0;
-    uint32_t x = v;                       // inclusive warp scan
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-      if ((int)lane_id() >= o) x += y;
-    }
-    if (lane_id() == 31) wsum[warp_id()] = x;
-    __syncthreads();
-    uint32_t woff = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; w++) {
-      if (w < (int)warp_id()) woff += wsum[w];
-      tot += wsum[w];
-    }
-    if (i < c.n_tiles) c.log_tilebase[i] = carry + woff + (x - v);
-    __syncthreads();
-    if (threadIdx.x == 0) carry += tot;
-    __syncthreads();
-  }
+  const unsigned long long end =
+      cta_exclusive_scan<unsigned long long>(c.log_tilecnt, c.log_tilebase, c.n_tiles, threadIdx.x == 0 ? c.log_total[0] : 0ull, wsum);
   if (threadIdx.x == 0) {
-    c.log_total[1] = carry;               // end ordinal of this chunk
-    c.log_total[0] = carry;               // base of the next chunk
+    c.log_total[1] = end;                 // end ordinal of this chunk
+    c.log_total[0] = end;                 // base of the next chunk
   }
 }
 
 // ---------------------------------------------------------------------------------------------------
 // K2 apply
 // ---------------------------------------------------------------------------------------------------
-template <int KIND, bool HAS_LOG>
+template <int KIND>
 __global__ void __launch_bounds__(kTile) k_apply(const Ctx c) {
   using W = Wire<KIND>;
   constexpr uint32_t NS = Stage<W::MSG>::N;
@@ -452,7 +439,7 @@ __global__ void __launch_bounds__(kTile) k_apply(const Ctx c) {
     {
       // listed requests: (a) the tile-segmented, index-ordered list (radix fallback of K3),
       //                  (b) the hash bucket K3 sorts in shared memory
-      const bool lg = HAS_LOG && valid && !ti.invalid && ti.is_log;
+      const bool lg = kHasLog<KIND> && valid && !ti.invalid && ti.is_log;
       uint32_t r_list, r_log, n_list, n_log;
       tile_rank2(listed, lg, scratch, r_list, r_log, n_list, n_log);
       if (lg) {
@@ -521,6 +508,40 @@ DINT_D void replay_run(const Ctx& c, const uint64_t* sorted, uint32_t p, uint32_
   if (len > 1) atomicMax(&c.counters[2], (unsigned long long)len);
 }
 
+// Replays the m sorted (group << 32 | index) keys, one same-group run after another in index order, by a team of
+// threads: one warp (ordered_buckets) or the whole grid (k_ordered).  A team has first() and stride() over the keys
+// and sync(), a barrier of the whole team.  FastReplay kinds take three passes -- every request's op into ops[p]
+// (in parallel), each run head walks its run with the group state in registers and leaves the replies in res[p],
+// then every reply is written (in parallel); the others replay each run request by request from its head.
+template <int KIND, class Team>
+DINT_D void replay_sorted_runs(const Ctx& c, const uint64_t* keys, uint32_t m, uint32_t* ops, uint64_t* res, Team& team) {
+  if constexpr (FastReplay<KIND>::ok) {
+    using FR = FastReplay<KIND>;
+    using W = Wire<KIND>;
+    for (uint32_t p = team.first(); p < m; p += team.stride()) ops[p] = FR::load_op(c.ord_req + (size_t)(uint32_t)keys[p] * W::MSG);
+    team.sync();
+    for (uint32_t p = team.first(); p < m; p += team.stride())
+      if (p == 0 || (uint32_t)(keys[p - 1] >> 32) != (uint32_t)(keys[p] >> 32)) {
+        const uint32_t g = (uint32_t)(keys[p] >> 32);
+        typename FR::State st = FR::load_state(c, g);
+        uint32_t q = p;
+        for (; q < m && (uint32_t)(keys[q] >> 32) == g; q++) res[q] = FR::step(st, ops[q]);
+        FR::store_state(c, g, st);
+        if (q - p > 1) atomicMax(&c.counters[2], (unsigned long long)(q - p));
+      }
+    team.sync();
+    for (uint32_t p = team.first(); p < m; p += team.stride()) FR::write_result(ord_out_ptr<W::MSG>(c, (uint32_t)keys[p]), res[p]);
+  } else {
+    for (uint32_t p = team.first(); p < m; p += team.stride())
+      if (p == 0 || (uint32_t)(keys[p - 1] >> 32) != (uint32_t)(keys[p] >> 32)) replay_run<KIND>(c, keys, p, m);
+  }
+}
+struct WarpTeam {                 // replay_sorted_runs by one warp (ordered_buckets)
+  DINT_D uint32_t first() const { return lane_id(); }
+  DINT_D uint32_t stride() const { return 32; }
+  DINT_D void sync() { __syncwarp(); }
+};
+
 // Ordered replay of the listed requests of a finished chunk (see engine.cuh).  Called by every warp of the
 // grid; `scratch` = blockDim.x/32 slices of OrdSlice<KIND>::BYTES.
 template <int KIND>
@@ -535,6 +556,7 @@ DINT_D void ordered_buckets(const Ctx& c, uint8_t* scratch) {
     uint64_t* wres = wkeys + kBucketCap;                       // fast replay only
     uint32_t* wops = (uint32_t*)(wkeys + 2 * kBucketCap);      // fast replay only
     const uint32_t lane = lane_id();
+    WarpTeam team;
     const uint32_t warps_per_cta = blockDim.x / 32;
     const uint32_t n_warps = gridDim.x * warps_per_cta;
     const uint32_t P = 1u << c.bucket_log2;
@@ -600,26 +622,7 @@ DINT_D void ordered_buckets(const Ctx& c, uint8_t* scratch) {
             }
         }
         __syncwarp();
-        if constexpr (FastReplay<KIND>::ok) {
-          using FR = FastReplay<KIND>;
-          using Wq = Wire<KIND>;
-          for (uint32_t p = lane; p < m; p += 32) wops[p] = FR::load_op(c.ord_req + (size_t)(uint32_t)wkeys[p] * Wq::MSG);
-          __syncwarp();
-          for (uint32_t p = lane; p < m; p += 32)
-            if (p == 0 || (uint32_t)(wkeys[p - 1] >> 32) != (uint32_t)(wkeys[p] >> 32)) {
-              const uint32_t g = (uint32_t)(wkeys[p] >> 32);
-              typename FR::State st = FR::load_state(c, g);
-              uint32_t q = p;
-              for (; q < m && (uint32_t)(wkeys[q] >> 32) == g; q++) wres[q] = FR::step(st, wops[q]);
-              FR::store_state(c, g, st);
-              if (q - p > 1) atomicMax(&c.counters[2], (unsigned long long)(q - p));
-            }
-          __syncwarp();
-          for (uint32_t p = lane; p < m; p += 32) FR::write_result(ord_out_ptr<Wq::MSG>(c, (uint32_t)wkeys[p]), wres[p]);
-        } else {
-          for (uint32_t p = lane; p < m; p += 32)
-            if (p == 0 || (uint32_t)(wkeys[p - 1] >> 32) != (uint32_t)(wkeys[p] >> 32)) replay_run<KIND>(c, wkeys, p, m);
-        }
+        replay_sorted_runs<KIND>(c, wkeys, m, wops, wres, team);
         __syncwarp();
       }
       if (lane < gsz && myb < P && cnt) c.bcnt[myb] = 0;
@@ -699,6 +702,12 @@ struct GridBar {
     __syncthreads();
   }
 };
+struct GridTeam {                 // replay_sorted_runs over the whole grid of k_ordered
+  GridBar& bar;
+  DINT_D uint32_t first() const { return blockIdx.x * kThreads + threadIdx.x; }
+  DINT_D uint32_t stride() const { return gridDim.x * kThreads; }
+  DINT_D void sync() { bar.sync(); }
+};
 
 template <int KIND>
 __global__ void __launch_bounds__(kThreads) k_ordered(const Ctx c) {
@@ -710,39 +719,13 @@ __global__ void __launch_bounds__(kThreads) k_ordered(const Ctx c) {
   GridBar grid{cg::this_grid(), c.gbar, c.coop_launch != 0};
   __shared__ uint64_t skeys[2048];                    // radix counters
   __shared__ uint32_t wsum[kThreads / 32];
-  __shared__ uint32_t s_carry;
   const uint32_t tid = threadIdx.x;
   const uint32_t P = 1u << c.bucket_log2;
   {
     // ---- fallback (skewed chunk): stable LSD radix sort of the whole list by group id --------------
     for (uint32_t b = blockIdx.x * kThreads + tid; b < P; b += gridDim.x * kThreads) c.bcnt[b] = 0;
     // (0) exclusive prefix of the per-tile list lengths (CTA 0)
-    if (blockIdx.x == 0) {
-      if (tid == 0) s_carry = 0;
-      __syncthreads();
-      for (uint32_t base = 0; base < c.n_tiles; base += kThreads) {
-        uint32_t i = base + tid;
-        uint32_t v = i < c.n_tiles ? c.ccnt[i] : 0;
-        uint32_t x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-          if ((int)lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) wsum[warp_id()] = x;
-        __syncthreads();
-        uint32_t woff = 0, tot = 0;
-#pragma unroll
-        for (int w = 0; w < kThreads / 32; w++) {
-          if (w < (int)warp_id()) woff += wsum[w];
-          tot += wsum[w];
-        }
-        if (i < c.n_tiles) c.cprefix[i] = s_carry + woff + (x - v);
-        __syncthreads();
-        if (tid == 0) s_carry += tot;
-        __syncthreads();
-      }
-    }
+    if (blockIdx.x == 0) (void)cta_exclusive_scan<uint32_t>(c.ccnt, c.cprefix, c.n_tiles, 0u, wsum);
     grid.sync();
     // (1) densify the tile-segmented list into (group << 32 | index), index-ascending
     for (uint32_t t = blockIdx.x; t < c.n_tiles; t += gridDim.x) {
@@ -798,34 +781,11 @@ __global__ void __launch_bounds__(kThreads) k_ordered(const Ctx c) {
         for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
         if (lane_id() == 0) wsum[warp_id()] = part;
         __syncthreads();
-        if (tid == 0) {
-          uint32_t b = 0;
+        uint32_t b = 0;                                          // digits below d, all tiles (thread 0)
+        if (tid == 0)
           for (int w = 0; w < kThreads / 32; w++) b += wsum[w];
-          s_carry = b;
-        }
-        __syncthreads();
-        for (uint32_t base = 0; base < n_st; base += kThreads) {
-          uint32_t T = base + tid;
-          uint32_t v = T < n_st ? c.ghist[(size_t)d * n_st + T] : 0;
-          uint32_t x = v;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) {
-            uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if ((int)lane_id() >= o) x += y;
-          }
-          if (lane_id() == 31) wsum[warp_id()] = x;
-          __syncthreads();
-          uint32_t woff = 0, tot = 0;
-#pragma unroll
-          for (int w = 0; w < kThreads / 32; w++) {
-            if (w < (int)warp_id()) woff += wsum[w];
-            tot += wsum[w];
-          }
-          if (T < n_st) c.ghist[(size_t)d * n_st + T] = s_carry + woff + (x - v);
-          __syncthreads();
-          if (tid == 0) s_carry += tot;
-          __syncthreads();
-        }
+        uint32_t* row = c.ghist + (size_t)d * n_st;
+        (void)cta_exclusive_scan<uint32_t>(row, row, n_st, b, wsum);
       }
       grid.sync();
       // (d) stable scatter: warp w owns items [w*256, w*256+256) of the tile, in 8 rounds of 32
@@ -978,32 +938,10 @@ __global__ void __launch_bounds__(kThreads) k_ordered(const Ctx c) {
           FR::store_state(c, g, st);
         }
       }
-    } else if constexpr (FastReplay<KIND>::ok) {
-      // replay in three passes: request fields of ALL listed requests (parallel) -> per-run walk with the
-      // group state in registers -> replies (parallel).  ops live in the (now free) clist, replies in `dst`.
-      using FR = FastReplay<KIND>;
-      using Wq = Wire<KIND>;
-      uint32_t* ops_g = c.clist;
-      uint64_t* res_g = dst;
-      for (uint32_t p = blockIdx.x * kThreads + tid; p < nc; p += gridDim.x * kThreads)
-        ops_g[p] = FR::load_op(c.ord_req + (size_t)(uint32_t)src[p] * Wq::MSG);
-      grid.sync();
-      for (uint32_t p = blockIdx.x * kThreads + tid; p < nc; p += gridDim.x * kThreads)
-        if (p == 0 || (uint32_t)(src[p - 1] >> 32) != (uint32_t)(src[p] >> 32)) {
-          const uint32_t g = (uint32_t)(src[p] >> 32);
-          typename FR::State st = FR::load_state(c, g);
-          uint32_t q = p;
-          for (; q < nc && (uint32_t)(src[q] >> 32) == g; q++) res_g[q] = FR::step(st, ops_g[q]);
-          FR::store_state(c, g, st);
-          if (q - p > 1) atomicMax(&c.counters[2], (unsigned long long)(q - p));
-        }
-      grid.sync();
-      for (uint32_t p = blockIdx.x * kThreads + tid; p < nc; p += gridDim.x * kThreads)
-        FR::write_result(ord_out_ptr<Wq::MSG>(c, (uint32_t)src[p]), res_g[p]);
     } else {
-      // replay: one thread per same-group run
-      for (uint32_t p = blockIdx.x * kThreads + tid; p < nc; p += gridDim.x * kThreads)
-        if (p == 0 || (uint32_t)(src[p - 1] >> 32) != (uint32_t)(src[p] >> 32)) replay_run<KIND>(c, src, p, nc);
+      // the sorted list, replayed by the whole grid: ops live in the (now free) clist, replies in `dst`
+      GridTeam team{grid};
+      replay_sorted_runs<KIND>(c, src, nc, c.clist, dst, team);
     }
   }
   if (blockIdx.x == 0 && tid == 0) atomicAdd(&c.counters[1], (unsigned long long)nc);

@@ -324,8 +324,8 @@ class ShardedEngine:
         return self._submit_gpu_exact(req, n, dst)
 
     def _submit_gpu_exact(self, req, n, dst):
-        """GPU path: dispatch / combine with the library's own kernels (k_route_owner, k_route_count/scan/scatter,
-        k_route_unpermute); NCCL moves the partitioned wire records."""
+        """GPU path: dispatch / combine with the library's own kernels (k_route_owner, k_exact_count/scan/scatter,
+        k_exact_unpermute); NCCL moves the partitioned wire records."""
         eng = self.engine
         owner = dst if dst is not None else eng.route_owner(req)
         send, perm, counts = eng.route_partition(req, owner, self.world)
