@@ -65,7 +65,19 @@ enum { KT_CLASSIFY = 0, KT_LOGSCAN, KT_APPLY, KT_ORDERED, KT_LOAD, KT_NUM };
 static const char* kKernelNames[KT_NUM] = {"k_classify", "k_log_scan", "k_apply", "k_ordered", "k_kv_load"};
 
 struct EvPair { cudaEvent_t a, b; int which; };
-constexpr int kHostBufs = 4;      // device staging buffers of the host path (dint_submit)
+constexpr int kHostBufs = 4;      // staging sets of dint_submit, and the most any host-path caller uses
+// Device staging of the host paths, dint_submit's slices and the multi-GPU step's batches: batch j of a call uses set
+// b = j % sets, with H2D on s_in and D2H on s_out next to the compute.  The caller records released[b] behind the last
+// launch that reads in[b] / aux[b], and makes the launch that writes out[b] wait for d2h[b] once j >= sets.
+// dint_submit and the step share the ring because one engine never has both in flight: dint_submit begins with a
+// device synchronise, and shard_run with host buffers ends by synchronising its copy and main streams.
+struct HostRing {
+  struct Buf { uint8_t* p = nullptr; size_t cap = 0; };
+  Buf in[kHostBufs], aux[kHostBufs], out[kHostBufs];   // requests | client-chosen destination bytes (the step) | replies
+  cudaEvent_t h2d[kHostBufs]{}, released[kHostBufs]{}, ready[kHostBufs]{}, d2h[kHostBufs]{};
+  cudaStream_t s_in = nullptr, s_out = nullptr;
+  uint32_t sets = 0;                                    // of the current call (buffers are allocated on first use, then only grow)
+};
 
 struct dint_engine {
   int kind = 0;
@@ -77,10 +89,8 @@ struct dint_engine {
   bool has_log = false;
   Ctx ctx{};                       // device pointers + constants; per-launch fields filled per chunk
   std::vector<void*> allocs;       // everything to cudaFree
-  cudaStream_t stream = nullptr, s_in = nullptr, s_out = nullptr;
-  uint8_t* d_req[kHostBufs] = {nullptr};
-  uint8_t* d_resp[kHostBufs] = {nullptr};
-  cudaEvent_t ev_in[kHostBufs]{}, ev_comp[kHostBufs]{}, ev_out[kHostBufs]{};
+  cudaStream_t stream = nullptr;
+  HostRing ring;                             // host-path staging of dint_submit and the multi-GPU step
   uint32_t host_chunk = 0;                   // requests per host-path slice
   bool plain_launches = false;               // inside the multi-GPU step: no cooperative launches (see GridBar)
   uint32_t host_min_slice = 0;               // smallest slice of the pyramid a host-path call is cut into
@@ -445,6 +455,45 @@ struct HostSlices {
   }
 };
 
+// ---- the host staging ring (HostRing) -----------------------------------------------------------------------------
+static int ring_reserve(dint_engine* e, uint32_t sets, size_t in_bytes, size_t aux_bytes, size_t out_bytes) {
+  HostRing& R = e->ring;
+  for (uint32_t b = 0; b < sets; b++) {
+    const std::pair<HostRing::Buf*, size_t> want[] = {{&R.in[b], in_bytes}, {&R.aux[b], aux_bytes}, {&R.out[b], out_bytes}};
+    for (auto [buf, bytes] : want)
+      if (bytes && buf->cap < bytes + 16) {
+        CU(cudaFree(buf->p));                 // too small for this call: no earlier call is in flight
+        *buf = HostRing::Buf{};
+        CU(cudaMalloc(&buf->p, bytes + 16));
+        buf->cap = bytes + 16;
+      }
+  }
+  R.sets = sets;
+  return DINT_OK;
+}
+static int ring_stage_in(dint_engine* e, uint64_t j, const void* host_in, size_t in_bytes, const void* host_aux, size_t aux_bytes, cudaStream_t consumer) {
+  HostRing& R = e->ring;
+  const uint32_t b = (uint32_t)(j % R.sets);
+  if (j >= R.sets) CU(cudaStreamWaitEvent(R.s_in, R.released[b], 0));
+  if (in_bytes) CU(cudaMemcpyAsync(R.in[b].p, host_in, in_bytes, cudaMemcpyHostToDevice, R.s_in));
+  if (aux_bytes) CU(cudaMemcpyAsync(R.aux[b].p, host_aux, aux_bytes, cudaMemcpyHostToDevice, R.s_in));
+  CU(cudaEventRecord(R.h2d[b], R.s_in));
+  CU(cudaStreamWaitEvent(consumer, R.h2d[b], 0));
+  e->stats.h2d_bytes += in_bytes + aux_bytes;
+  return DINT_OK;
+}
+// batch j's replies are final behind what `producer` has enqueued so far
+static int ring_drain_out(dint_engine* e, uint64_t j, void* host_out, size_t out_bytes, cudaStream_t producer) {
+  HostRing& R = e->ring;
+  const uint32_t b = (uint32_t)(j % R.sets);
+  CU(cudaEventRecord(R.ready[b], producer));
+  CU(cudaStreamWaitEvent(R.s_out, R.ready[b], 0));
+  if (out_bytes) CU(cudaMemcpyAsync(host_out, R.out[b].p, out_bytes, cudaMemcpyDeviceToHost, R.s_out));
+  CU(cudaEventRecord(R.d2h[b], R.s_out));
+  e->stats.d2h_bytes += out_bytes;
+  return DINT_OK;
+}
+
 // ---- fused dispatch / combine (route.cuh) ---------------------------------------------------------------
 template <int KIND>
 static int route_dispatch_t(dint_engine* e, const RouteArgs& a, cudaStream_t s) {
@@ -533,14 +582,12 @@ void dint_destroy(dint_engine* e) {
   if (e->h_kvcnt) cudaFreeHost(e->h_kvcnt);
   if (e->ev_kvcnt) cudaEventDestroy(e->ev_kvcnt);
   for (auto& ep : e->ev_pool) { cudaEventDestroy(ep.a); cudaEventDestroy(ep.b); }
+  HostRing& R = e->ring;
   for (int i = 0; i < kHostBufs; i++) {
-    if (e->ev_in[i]) cudaEventDestroy(e->ev_in[i]);
-    if (e->ev_comp[i]) cudaEventDestroy(e->ev_comp[i]);
-    if (e->ev_out[i]) cudaEventDestroy(e->ev_out[i]);
+    for (HostRing::Buf* b : {&R.in[i], &R.aux[i], &R.out[i]}) cudaFree(b->p);
+    for (cudaEvent_t ev : {R.h2d[i], R.released[i], R.ready[i], R.d2h[i]}) if (ev) cudaEventDestroy(ev);
   }
-  if (e->stream) cudaStreamDestroy(e->stream);
-  if (e->s_in) cudaStreamDestroy(e->s_in);
-  if (e->s_out) cudaStreamDestroy(e->s_out);
+  for (cudaStream_t s : {e->stream, R.s_in, R.s_out}) if (s) cudaStreamDestroy(s);
   delete e;
 }
 
@@ -549,13 +596,10 @@ static int create_impl(dint_engine* e) {
   Ctx& c = e->ctx;
   CU(cudaSetDevice(e->device));
   CU(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-  for (int i = 0; i < kHostBufs; i++) {
-    CU(cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&e->ev_comp[i], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming));
-  }
+  HostRing& R = e->ring;
+  for (cudaStream_t* s : {&R.s_in, &R.s_out}) CU(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
+  for (int i = 0; i < kHostBufs; i++)
+    for (cudaEvent_t* ev : {&R.h2d[i], &R.released[i], &R.ready[i], &R.d2h[i]}) CU(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
   c.n_shards = cf.n_shards;
   c.shard_id = cf.shard_id;
   c.shard_div = make_fastmod(cf.n_shards);
@@ -846,35 +890,25 @@ int dint_submit_device(dint_engine* e, const void* req_dev, uint64_t n, void* re
 int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
   if (!e || (n && (!req || !resp))) return set_err(DINT_EINVAL, "null argument");
   CU(cudaSetDevice(e->device));
-  // the host path moves data in slices of `hchunk` requests through a ring of kHostBufs device buffers:
+  // the host path moves data in slices of `hchunk` requests through the engine's ring of kHostBufs staging sets:
   // small slices keep the PCIe fill/drain bubbles short, the ring keeps both copy engines and the SMs busy
   const uint32_t hchunk = e->host_chunk;
-  if (!e->d_req[0]) {
-    for (int i = 0; i < kHostBufs; i++) {
-      int rc;
-      if ((rc = dalloc(e, &e->d_req[i], (size_t)hchunk * e->msg + 16, false))) return rc;
-      if ((rc = dalloc(e, &e->d_resp[i], (size_t)hchunk * e->msg + 16, false))) return rc;
-    }
-  }
   static const bool trace = getenv("DINT_HOST_TRACE") != nullptr;
   const auto t_begin = std::chrono::steady_clock::now();
   CU(cudaDeviceSynchronize());     // order after anything submitted on user streams
+  { int rc = ring_reserve(e, kHostBufs, (size_t)hchunk * e->msg, 0, (size_t)hchunk * e->msg); if (rc) return rc; }
   { int rc = kv_maintain(e, e->stream); if (rc) return rc; }
   const uint8_t* rq = (const uint8_t*)req;
   uint8_t* rs = (uint8_t*)resp;
   unsigned long long err_before = e->stats.errors;
-  // three-stage pipeline: H2D (s_in) | kernels (stream) | D2H (s_out).  Slice k's replies are final only
+  // three-stage pipeline: H2D (ring s_in) | kernels (stream) | D2H (ring s_out).  Slice k's replies are final only
   // after the launch that replays its listed requests -- K1 of slice k+1, or the flush after the last
-  // slice -- so D2H(k) is ordered behind that.
+  // slice -- so D2H(k) is ordered behind that.  That launch is also the last to read slice k's requests.
   uint64_t k = 0;
   uint64_t prev_off = 0, prev_bytes = 0;
   auto copy_out_prev = [&](uint64_t kk) -> int {          // D2H of slice kk-1
-    int pb = (int)((kk - 1) % kHostBufs);
-    CU(cudaEventRecord(e->ev_comp[pb], e->stream));
-    CU(cudaStreamWaitEvent(e->s_out, e->ev_comp[pb], 0));
-    CU(cudaMemcpyAsync(rs + prev_off, e->d_resp[pb], prev_bytes, cudaMemcpyDeviceToHost, e->s_out));
-    CU(cudaEventRecord(e->ev_out[pb], e->s_out));
-    return DINT_OK;
+    CU(cudaEventRecord(e->ring.released[(kk - 1) % kHostBufs], e->stream));
+    return ring_drain_out(e, kk - 1, rs + prev_off, prev_bytes, e->stream);
   };
   // Slice schedule.  PCIe moves large copies better than small ones (tools/pcie_probe.cu measures it), but the
   // first slice's H2D and the last two slices' kernels + D2H overlap with nothing.  So a call is cut as a
@@ -884,18 +918,13 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
   for (uint64_t cn; (cn = sched.next()) != 0; k++) {
     int b = (int)(k % kHostBufs);
     size_t bytes = (size_t)cn * e->msg;
-    if (k >= (uint64_t)kHostBufs) CU(cudaStreamWaitEvent(e->s_in, e->ev_comp[b], 0));   // slice k-kHostBufs no longer read
-    CU(cudaMemcpyAsync(e->d_req[b], rq + off * e->msg, bytes, cudaMemcpyHostToDevice, e->s_in));
-    CU(cudaEventRecord(e->ev_in[b], e->s_in));
-    CU(cudaStreamWaitEvent(e->stream, e->ev_in[b], 0));
-    if (k >= (uint64_t)kHostBufs) CU(cudaStreamWaitEvent(e->stream, e->ev_out[b], 0)); // its replies have left d_resp[b]
-    int rc = submit_chunk(e, e->d_req[b], (uint32_t)cn, e->d_resp[b], e->stream);
+    if (k >= (uint64_t)kHostBufs) CU(cudaStreamWaitEvent(e->stream, e->ring.d2h[b], 0));     // slice k-kHostBufs's replies have left out[b]
+    int rc = ring_stage_in(e, k, rq + off * e->msg, bytes, nullptr, 0, e->stream);
+    if (!rc) rc = submit_chunk(e, e->ring.in[b].p, (uint32_t)cn, e->ring.out[b].p, e->stream);
     if (rc) return rc;
     if (k >= 1 && (rc = copy_out_prev(k))) return rc;                   // slice k-1 is final now
     prev_off = off * e->msg;
     prev_bytes = bytes;
-    e->stats.h2d_bytes += bytes;
-    e->stats.d2h_bytes += bytes;
     off += cn;
   }
   {
@@ -907,7 +936,7 @@ int dint_submit(dint_engine* e, const void* req, uint64_t n, void* resp) {
   CU(cudaMemcpyAsync(e->h_counters, e->ctx.counters, kNumCounters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
   { int rc2 = kv_publish_counts(e, e->stream); if (rc2) return rc2; }
   const auto t_enq = std::chrono::steady_clock::now();
-  CU(cudaStreamSynchronize(e->s_out));
+  CU(cudaStreamSynchronize(e->ring.s_out));
   CU(cudaStreamSynchronize(e->stream));
   int rc = prof_flush(e);
   if (rc) return rc;
@@ -1153,6 +1182,7 @@ int64_t dint_kv_count(dint_engine* e, int table) {
 // dint_shard_*) or in ONE process (dint_cluster_*: cudaMalloc + peer access; several ranks may even share a
 // device, then everything runs on one stream in dependency order).
 constexpr int kMaxSets = 4;
+static_assert(kMaxSets <= kHostBufs, "the host path stages batch j in set j % n_sets of the engine's HostRing");
 struct dint_shard_ctx {
   dint_engine* e = nullptr;
   uint32_t W = 0, me = 0, cap = 0, S = 0;
@@ -1160,12 +1190,10 @@ struct dint_shard_ctx {
   PeerPtrs sigreq{}, sigrsp{};
   uint32_t *my_req = nullptr, *my_rsp = nullptr;
   uint32_t epoch = 0;
-  cudaStream_t side = nullptr, ret = nullptr, s_in = nullptr, s_out = nullptr;
+  cudaStream_t side = nullptr, ret = nullptr;
   cudaEvent_t ev_disp[kMaxSets]{}, ev_comb[kMaxSets]{}, ev_fork = nullptr;
-  cudaEvent_t ev_h2d[kMaxSets]{}, ev_d2h[kMaxSets]{};
   uint8_t* owner[kMaxSets]{};
   uint32_t* tilebase[kMaxSets]{};
-  uint8_t *st_req[kMaxSets]{}, *st_dst[kMaxSets]{}, *st_out[kMaxSets]{};   // host-path staging (allocated on first use)
   uint32_t* flags = nullptr;
   uint64_t max_n = 0;
   bool one_stream = false;                 // ranks sharing a device: dispatch, engine and combine on ONE stream, in dependency order
@@ -1200,16 +1228,12 @@ static int shard_make(dint_engine* e, uint32_t n_shards, uint32_t rank, uint32_t
     CU(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking));
     CU(cudaStreamCreateWithFlags(&c->ret, cudaStreamNonBlocking));
   }
-  CU(cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
   CU(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
   const uint32_t tr = route_tile_records(e);
   const size_t tiles = (size_t)((max_n + tr - 1) / tr);
   for (uint32_t s = 0; s < n_sets; s++) {
     CU(cudaEventCreateWithFlags(&c->ev_disp[s], cudaEventDisableTiming));
     CU(cudaEventCreateWithFlags(&c->ev_comb[s], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&c->ev_h2d[s], cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&c->ev_d2h[s], cudaEventDisableTiming));
     CU(cudaMalloc(&c->owner[s], max_n + 16));
     CU(cudaMalloc(&c->tilebase[s], tiles * kMaxShards * sizeof(uint32_t)));
   }
@@ -1301,18 +1325,8 @@ static void shard_trace_collect(dint_shard_ctx* c, uint32_t k) {
 // before it, on this or another GPU, so one host thread can drive all ranks without blocking.
 struct ShardBatch { const void* req; const uint8_t* dst; void* out; uint64_t n; uint32_t cap = 0; };   // cap: slab records of this batch (0 = the full capacity)
 struct HostBatch { const uint8_t* req; const uint8_t* dst; uint8_t* out; uint64_t n; };
-static int shard_staging(dint_shard_ctx* c) {
-  if (c->st_req[0]) return DINT_OK;
-  CU(cudaSetDevice(c->e->device));
-  for (uint32_t s = 0; s < c->S; s++) {
-    CU(cudaMalloc(&c->st_req[s], c->max_n * c->e->msg + 16));
-    CU(cudaMalloc(&c->st_dst[s], c->max_n + 16));
-    CU(cudaMalloc(&c->st_out[s], c->max_n * c->e->msg + 16));
-  }
-  return DINT_OK;
-}
-// `host` given: the batches come from / go to HOST memory through S staging sets -- H2D of batch j+1 (copy stream) and
-// D2H of batch j-1 (another copy stream) run next to the exchange of batch j, the same slice ring as dint_submit.
+// `host` given: the batches come from / go to HOST memory through S sets of each rank's engine ring (HostRing) --
+// H2D of batch j+1 and D2H of batch j-1 run on the ring's copy streams next to the exchange of batch j.
 static int shard_run(dint_shard_ctx* const* ranks, uint32_t R, uint32_t k, std::vector<std::vector<ShardBatch>>& b, cudaStream_t const* mains,
                      const std::vector<std::vector<HostBatch>>* host = nullptr) {
   if (k == 0) return DINT_OK;
@@ -1321,9 +1335,9 @@ static int shard_run(dint_shard_ctx* const* ranks, uint32_t R, uint32_t k, std::
   int rc;
   for (uint32_t r = 0; r < R; r++) {
     dint_shard_ctx* c = ranks[r];
-    if (host && (rc = shard_staging(c))) return rc;
-    if (one) continue;
     CU(cudaSetDevice(c->e->device));
+    if (host && (rc = ring_reserve(c->e, c->S, c->max_n * c->e->msg, c->max_n, c->max_n * c->e->msg))) return rc;
+    if (one) continue;
     CU(cudaEventRecord(c->ev_fork, mains[r]));
     CU(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
     CU(cudaStreamWaitEvent(c->ret, c->ev_fork, 0));
@@ -1332,34 +1346,25 @@ static int shard_run(dint_shard_ctx* const* ranks, uint32_t R, uint32_t k, std::
   auto retS = [&](uint32_t r) { return one ? mains[r] : ranks[r]->ret; };
   auto dispatch = [&](uint32_t r, uint32_t j) -> int {
     dint_shard_ctx* c = ranks[r];
-    if (host) {                                          // stage batch j: H2D on the copy stream, the dispatch waits for it
+    if (host) {                                          // stage batch j: H2D on the ring's copy stream, the dispatch waits for it
       const HostBatch& h = (*host)[r][j];
       dint_engine* e = c->e;
       const uint32_t s = j % c->S;
       if (h.n > c->max_n) return set_err(DINT_EINVAL, "batch size");
       CU(cudaSetDevice(e->device));
-      CU(cudaStreamWaitEvent(c->s_in, c->ev_d2h[s], 0)); // batch j - S has left this staging set (its dispatch is long done too)
-      if (h.n) CU(cudaMemcpyAsync(c->st_req[s], h.req, h.n * e->msg, cudaMemcpyHostToDevice, c->s_in));
-      if (h.dst && h.n) CU(cudaMemcpyAsync(c->st_dst[s], h.dst, h.n, cudaMemcpyHostToDevice, c->s_in));
-      CU(cudaEventRecord(c->ev_h2d[s], c->s_in));
-      CU(cudaStreamWaitEvent(side(r), c->ev_h2d[s], 0));
-      e->stats.h2d_bytes += h.n * e->msg + (h.dst ? h.n : 0);
-      b[r][j] = ShardBatch{c->st_req[s], h.dst ? c->st_dst[s] : nullptr, c->st_out[s], h.n, 0};
+      if (int rc2 = ring_stage_in(e, j, h.req, h.n * e->msg, h.dst, h.dst ? h.n : 0, side(r))) return rc2;
+      b[r][j] = ShardBatch{e->ring.in[s].p, h.dst ? e->ring.aux[s].p : nullptr, e->ring.out[s].p, h.n, 0};
     }
-    return shard_dispatch(c, j, c->epoch + 1 + j, b[r][j].req, b[r][j].dst, b[r][j].n, b[r][j].cap ? b[r][j].cap : c->cap, side(r));
+    int rc2 = shard_dispatch(c, j, c->epoch + 1 + j, b[r][j].req, b[r][j].dst, b[r][j].n, b[r][j].cap ? b[r][j].cap : c->cap, side(r));
+    if (!rc2 && host) CU(cudaEventRecord(c->e->ring.released[j % c->S], side(r)));   // nothing after the dispatch reads in / aux
+    return rc2;
   };
   auto combine = [&](uint32_t r, uint32_t j) -> int {
     dint_shard_ctx* c = ranks[r];
+    if (host && j >= c->S) CU(cudaStreamWaitEvent(retS(r), c->e->ring.d2h[j % c->S], 0));   // batch j - S's replies have left out[j % S]
     int rc2 = shard_combine(c, j, c->epoch + 1 + j, b[r][j].out, b[r][j].n, b[r][j].cap ? b[r][j].cap : c->cap, retS(r));
     if (rc2 || !host) return rc2;
-    const HostBatch& h = (*host)[r][j];
-    const uint32_t s = j % c->S, es = (c->epoch + 1 + j) % c->S;
-    if (one) CU(cudaEventRecord(c->ev_comb[es], retS(r)));
-    CU(cudaStreamWaitEvent(c->s_out, c->ev_comb[es], 0));
-    if (h.n) CU(cudaMemcpyAsync(h.out, c->st_out[s], h.n * c->e->msg, cudaMemcpyDeviceToHost, c->s_out));
-    CU(cudaEventRecord(c->ev_d2h[s], c->s_out));
-    c->e->stats.d2h_bytes += h.n * c->e->msg;
-    return DINT_OK;
+    return ring_drain_out(c->e, j, (*host)[r][j].out, (*host)[r][j].n * c->e->msg, retS(r));
   };
   for (uint32_t r = 0; r < R; r++)
     if ((rc = dispatch(r, 0))) return rc;
@@ -1389,7 +1394,7 @@ static int shard_run(dint_shard_ctx* const* ranks, uint32_t R, uint32_t k, std::
   if (host)
     for (uint32_t r = 0; r < R; r++) {                   // returns when every reply is in host memory
       CU(cudaSetDevice(ranks[r]->e->device));
-      CU(cudaStreamSynchronize(ranks[r]->s_out));
+      CU(cudaStreamSynchronize(ranks[r]->e->ring.s_out));
       CU(cudaStreamSynchronize(mains[r]));
     }
   for (uint32_t r = 0; r < R; r++) shard_trace_collect(ranks[r], k);
@@ -1424,20 +1429,13 @@ void dint_shard_destroy(dint_shard_ctx* c) {
   for (uint32_t s = 0; s < c->S; s++) {
     if (c->ev_disp[s]) cudaEventDestroy(c->ev_disp[s]);
     if (c->ev_comb[s]) cudaEventDestroy(c->ev_comb[s]);
-    if (c->ev_h2d[s]) cudaEventDestroy(c->ev_h2d[s]);
-    if (c->ev_d2h[s]) cudaEventDestroy(c->ev_d2h[s]);
     if (c->owner[s]) cudaFree(c->owner[s]);
     if (c->tilebase[s]) cudaFree(c->tilebase[s]);
-    if (c->st_req[s]) cudaFree(c->st_req[s]);
-    if (c->st_dst[s]) cudaFree(c->st_dst[s]);
-    if (c->st_out[s]) cudaFree(c->st_out[s]);
   }
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->flags) cudaFree(c->flags);
   if (c->side) cudaStreamDestroy(c->side);
   if (c->ret) cudaStreamDestroy(c->ret);
-  if (c->s_in) cudaStreamDestroy(c->s_in);
-  if (c->s_out) cudaStreamDestroy(c->s_out);
   c->e->plain_launches = false;
   delete c;
 }
