@@ -16,6 +16,7 @@
 #include "route.cuh"
 #include "kv.cuh"
 #include "clients.cuh"
+#include "txn_clients.cuh"
 
 using namespace dint;
 
@@ -1797,6 +1798,275 @@ int dint_clients_peek(dint_clients* c, void* next_req_host, void* last_resp_host
   }
   if (next_req_host) CU(cudaMemcpy(next_req_host, c->req, (size_t)c->cc.n_clients * 9, cudaMemcpyDeviceToHost));
   if (last_resp_host) CU(cudaMemcpy(last_resp_host, c->resp, (size_t)c->cc.n_clients * 9, cudaMemcpyDeviceToHost));
+  return DINT_OK;
+}
+
+}  // extern "C"
+
+extern "C" {
+// ---- TATP / SmallBank closed-loop clients on the GPU against a shard cluster (txn_clients.cuh) ---------------
+// The clients are split over the cluster's ranks in contiguous blocks of gids, rank r's block on rank r's device, so
+// rank-major order is global client order and every shard sees its records in the order one host TxnWorkload would
+// send them.  A round: the step / scan / compact kernels leave the round in req[] / dst[] on every rank and its size
+// and per-shard counts in a pinned block; ONE event synchronise per rank hands those G x (G + 1) words to the host,
+// which sizes the exchange slabs exactly from them and serves the round with one shard_run on device buffers; the
+// clients' next step absorbs the replies straight from out[].  No record crosses PCIe.
+struct TxnRank {
+  txn::DevClients d{};
+  uint32_t tiles = 0;
+  uint8_t* out = nullptr;        // replies of the round, in the order of req[]
+  uint32_t* pub = nullptr;       // host view of d.pub: [0] records, [1 + o] records for shard o, [9..10] exchange flags
+  cudaEvent_t ev = nullptr;      // this rank's emission of the pending round is done
+  uint64_t last_n = 0;           // records of the last round served
+};
+struct dint_txn_clients {
+  dint_cluster* cl = nullptr;
+  uint32_t msg = 0, n = 0;
+  std::vector<TxnRank> rk;
+  std::vector<cudaStream_t> mains;
+  bool started = false;
+  uint64_t requests = 0, rounds = 0, fallback_rounds = 0;
+  cudaEvent_t t_beg = nullptr, t_end = nullptr;   // on rank 0's stream: the device work of one round
+  uint64_t timed = 0;
+  double wall_s = 0, dev_s = 0;
+};
+
+void dint_txn_clients_destroy(dint_txn_clients* t) {
+  if (!t) return;
+  for (size_t r = 0; r < t->rk.size(); r++) {
+    TxnRank& k = t->rk[r];
+    cudaSetDevice(t->cl->dev[r]);
+    cudaDeviceSynchronize();
+    cudaFree(k.d.cl); cudaFree(k.d.stg); cudaFree(k.d.stg_dst); cudaFree(k.d.cnt); cudaFree(k.d.off); cudaFree(k.d.tile_sum);
+    cudaFree(k.d.owner_cnt); cudaFree(k.d.stats); cudaFree(k.d.req); cudaFree(k.d.dst); cudaFree(k.out);
+    if (k.pub) cudaFreeHost(k.pub);
+    if (k.ev) cudaEventDestroy(k.ev);
+  }
+  if (!t->rk.empty()) cudaSetDevice(t->cl->dev[0]);
+  if (t->t_beg) cudaEventDestroy(t->t_beg);
+  if (t->t_end) cudaEventDestroy(t->t_end);
+  delete t;
+}
+
+int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0, uint32_t subscribers, dint_txn_clients** out) {
+  if (!cl || !out) return set_err(DINT_EINVAL, "null argument");
+  *out = nullptr;
+  if ((cl->kind != DINT_TATP && cl->kind != DINT_SMALLBANK) || n_clients == 0 || subscribers < 3)
+    return set_err(DINT_EINVAL, "a tatp or smallbank cluster, n_clients > 0, subscribers >= 3");
+  // fallback pieces start at multiples of 16 records, so that every device batch stays 16-byte aligned
+  if (((cl->cap < cl->max_n ? cl->cap : cl->max_n) & ~15ull) == 0) return set_err(DINT_EINVAL, "the cluster's max_batch must be >= 16");
+  const uint32_t G = cl->G, msg = kMsgSize[cl->kind];
+  dint_txn_clients* t = new dint_txn_clients();
+  t->cl = cl; t->msg = msg; t->n = n_clients;
+  txn::Cfg w{G, subscribers, 0};
+  if (cl->kind == DINT_SMALLBANK) {
+    w.hot = (uint32_t)((uint64_t)subscribers * 960000 / 24000000);   // kHotAccountNum / kAccountNum, as txn_workloads.cc
+    if (w.hot < 2) w.hot = 2;
+  }
+  const size_t csz = cl->kind == DINT_TATP ? sizeof(txn::TatpClient) : sizeof(txn::SbClient);
+  auto fail = [&](int code, const char* what, cudaError_t ce) { std::string keep; set_err(code, what, ce); keep = g_last_error;
+                                                               dint_txn_clients_destroy(t); g_last_error = keep; return code; };
+  t->rk.resize(G);
+  for (uint32_t r = 0; r < G; r++) {
+    TxnRank& k = t->rk[r];
+    const uint32_t lo = (uint32_t)((uint64_t)n_clients * r / G), hi = (uint32_t)((uint64_t)n_clients * (r + 1) / G);
+    const size_t n = hi - lo;
+    k.d.n = (uint32_t)n; k.d.gid0 = (uint64_t)gid0 + lo; k.d.w = w;
+    k.tiles = (uint32_t)((n + kThreads - 1) / kThreads);
+    t->mains.push_back(cl->shared_device ? cl->eng[0]->stream : cl->eng[r]->stream);
+    cudaError_t ce = cudaSetDevice(cl->dev[r]);
+    const size_t rec = n * txn::kMaxRecords;
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.cl, n * csz + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.stg, rec * msg + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.stg_dst, rec + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.cnt, n * 4 + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.off, n * 4 + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.tile_sum, (size_t)k.tiles * 4 + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.owner_cnt, 8 * sizeof(uint32_t));
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.stats, 14 * sizeof(unsigned long long));
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.req, rec * msg + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.dst, rec + 16);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.out, rec * msg + 16);
+    if (ce == cudaSuccess) ce = cudaHostAlloc(&k.pub, 16 * sizeof(uint32_t), cudaHostAllocMapped | cudaHostAllocPortable);
+    if (ce != cudaSuccess) return fail(DINT_ENOMEM, "txn client state", ce);
+    memset(k.pub, 0, 16 * sizeof(uint32_t));
+    if (ce == cudaSuccess) ce = cudaHostGetDevicePointer((void**)&k.d.pub, k.pub, 0);
+    if (ce == cudaSuccess) ce = cudaMemset(k.d.cl, 0, n * csz + 16);
+    if (ce == cudaSuccess) ce = cudaMemset(k.d.owner_cnt, 0, 8 * sizeof(uint32_t));
+    if (ce == cudaSuccess) ce = cudaMemset(k.d.stats, 0, 14 * sizeof(unsigned long long));
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&k.ev, cudaEventDisableTiming);
+    if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
+    if (ce != cudaSuccess) return fail(DINT_EIO, "txn client setup", ce);
+  }
+  cudaError_t ce = cudaSetDevice(cl->dev[0]);
+  if (ce == cudaSuccess) ce = cudaEventCreate(&t->t_beg);
+  if (ce == cudaSuccess) ce = cudaEventCreate(&t->t_end);
+  if (ce != cudaSuccess) return fail(DINT_EIO, "txn client events", ce);
+  *out = t;
+  return DINT_OK;
+}
+
+// enqueue one emission (step, scan, compact) on every rank; first = the clients start their first transactions
+static int txn_emit(dint_txn_clients* t, int first) {
+  dint_cluster* cl = t->cl;
+  for (uint32_t r = 0; r < cl->G; r++) {
+    TxnRank& k = t->rk[r];
+    CU(cudaSetDevice(cl->dev[r]));
+    const cudaStream_t s = t->mains[r];
+    if (k.d.n) {
+      if (cl->kind == DINT_TATP) txn::k_txn_step<DINT_TATP><<<k.tiles, kThreads, 0, s>>>(k.d, k.out, first);
+      else txn::k_txn_step<DINT_SMALLBANK><<<k.tiles, kThreads, 0, s>>>(k.d, k.out, first);
+      txn::k_txn_scan<<<1, kThreads, 0, s>>>(k.d, k.tiles);
+      if (cl->kind == DINT_TATP) txn::k_txn_compact<txn::TM><<<k.tiles, kThreads, 0, s>>>(k.d);
+      else txn::k_txn_compact<txn::SMSZ><<<k.tiles, kThreads, 0, s>>>(k.d);
+      cl->eng[r]->stats.kernel_launches += 3;
+    }
+    CU(cudaEventRecord(k.ev, s));
+  }
+  CU(cudaGetLastError());
+  t->started = true;
+  return DINT_OK;
+}
+// wait for every rank's pending emission; the exchange flags of the round before it must read zero
+static int txn_wait(dint_txn_clients* t) {
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    CU(cudaSetDevice(t->cl->dev[r]));
+    CU(cudaEventSynchronize(t->rk[r].ev));
+  }
+  for (uint32_t r = 0; r < t->cl->G; r++)
+    if (t->rk[r].pub[9] || t->rk[r].pub[10]) return set_err(DINT_EIO, "internal: an exchange slab overflowed or a wait timed out");
+  return DINT_OK;
+}
+static int txn_errors(dint_txn_clients* t, unsigned long long* sum) {
+  *sum = 0;
+  for (auto* e : t->cl->eng) {
+    CU(cudaSetDevice(e->device));
+    int rc = pull_counters(e);
+    if (rc) return rc;
+    *sum += e->stats.errors;
+  }
+  return DINT_OK;
+}
+
+int dint_txn_clients_run(dint_txn_clients* t, uint32_t rounds) {
+  if (!t) return set_err(DINT_EINVAL, "null argument");
+  dint_cluster* cl = t->cl;
+  const uint32_t G = cl->G, msg = t->msg;
+  unsigned long long err_before = 0, err_after = 0;
+  int rc = txn_errors(t, &err_before);
+  if (rc) return rc;
+  if (!t->started && (rc = txn_emit(t, 1))) return rc;
+  if ((rc = txn_wait(t))) return rc;
+  const uint32_t piece = (uint32_t)((cl->cap < cl->max_n ? cl->cap : cl->max_n) & ~15ull);
+  auto round_up = [](uint64_t x) { return (uint32_t)(x ? (x + kTile - 1) / kTile * kTile : kTile); };
+  std::vector<uint64_t> n(G);
+  std::vector<std::vector<ShardBatch>> b;
+  auto t_prev = std::chrono::steady_clock::now();
+  for (uint32_t i = 0; i < rounds; i++) {
+    // the slab capacity of the round: the largest (source, owner) count, so no slab can overflow
+    uint64_t maxc = 0;
+    bool fits = true;
+    for (uint32_t r = 0; r < G; r++) {
+      n[r] = t->rk[r].pub[0];
+      if (n[r] > cl->max_n) fits = false;
+      for (uint32_t o = 0; o < G; o++) maxc = t->rk[r].pub[1 + o] > maxc ? t->rk[r].pub[1 + o] : maxc;
+    }
+    if (maxc > cl->cap) fits = false;
+    b.assign(G, {});
+    if (fits) {
+      for (uint32_t r = 0; r < G; r++) b[r].push_back(ShardBatch{t->rk[r].d.req, t->rk[r].d.dst, t->rk[r].out, n[r], round_up(maxc)});
+    } else {
+      // one source rank at a time sends pieces of at most min(cap, max_n) records, the others send empty batches:
+      // every shard still sees rank-major order, and a piece this small cannot overflow a slab
+      t->fallback_rounds++;
+      for (uint32_t src = 0; src < G; src++)
+        for (uint64_t from = 0; from < n[src]; from += piece) {
+          const uint64_t len = n[src] - from < piece ? n[src] - from : piece;
+          for (uint32_t r = 0; r < G; r++) {
+            const TxnRank& k = t->rk[r];
+            b[r].push_back(r == src ? ShardBatch{k.d.req + from * msg, k.d.dst + from, k.out + from * msg, len, round_up(len)}
+                                    : ShardBatch{k.d.req, k.d.dst, k.out, 0, round_up(len)});
+          }
+        }
+    }
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventRecord(t->t_beg, t->mains[0]));
+    const uint32_t k = (uint32_t)b[0].size();
+    if (k && (rc = shard_run(cl->sh.data(), G, k, b, t->mains.data()))) return rc;
+    for (uint32_t r = 0; r < G; r++) {          // the exchange flags of this round (dint_shard_flags, without its synchronise)
+      CU(cudaSetDevice(cl->dev[r]));
+      CU(cudaMemcpyAsync(t->rk[r].pub + 9, cl->sh[r]->flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, t->mains[r]));
+      CU(cudaMemsetAsync(cl->sh[r]->flags, 0, 2 * sizeof(uint32_t), t->mains[r]));
+    }
+    for (uint32_t r = 0; r < G; r++) { t->rk[r].last_n = n[r]; t->requests += n[r]; }
+    t->rounds++;
+    if ((rc = txn_emit(t, 0))) return rc;
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventRecord(t->t_end, t->mains[0]));
+    if ((rc = txn_wait(t))) return rc;
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventSynchronize(t->t_end));
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, t->t_beg, t->t_end));
+    const auto now = std::chrono::steady_clock::now();
+    t->wall_s += std::chrono::duration<double>(now - t_prev).count();
+    t->dev_s += ms * 1e-3;
+    t->timed++;
+    t_prev = now;
+  }
+  if ((rc = txn_errors(t, &err_after))) return rc;
+  return err_after != err_before ? set_err(DINT_EPROTO, "an engine answered a request with an error reply") : DINT_OK;
+}
+
+// out: dint_txn_stats' 18 words (requests and rounds served, transactions started, committed, started-by-type[7],
+// committed-by-type[7]), then rounds served through the fallback
+int dint_txn_clients_stats(dint_txn_clients* t, uint64_t out[19]) {
+  if (!t || !out) return set_err(DINT_EINVAL, "null argument");
+  if (!t->started) { int rc = txn_emit(t, 1); if (rc) return rc; }
+  unsigned long long by[14] = {0};
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    unsigned long long h[14];
+    CU(cudaSetDevice(t->cl->dev[r]));
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(h, t->rk[r].d.stats, sizeof h, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < 14; i++) by[i] += h[i];
+  }
+  out[0] = t->requests; out[1] = 0; out[2] = 0; out[3] = t->rounds;
+  for (int i = 0; i < 7; i++) {
+    out[4 + i] = by[i]; out[11 + i] = by[7 + i];
+    out[1] += by[i]; out[2] += by[7 + i];
+  }
+  out[18] = t->fallback_rounds;
+  return DINT_OK;
+}
+
+// test hook, global client order: the pending round (its requests and destination shards) and the replies the clients
+// absorbed last; buffers of n_clients * 9 records
+int dint_txn_clients_peek(dint_txn_clients* t, void* next_req, uint8_t* next_dst, uint64_t* n_next, void* last_resp, uint64_t* n_last) {
+  if (!t) return set_err(DINT_EINVAL, "null argument");
+  int rc;
+  if (!t->started && (rc = txn_emit(t, 1))) return rc;
+  if ((rc = txn_wait(t))) return rc;
+  uint64_t a = 0, z = 0;
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    const TxnRank& k = t->rk[r];
+    const uint64_t n = k.pub[0];
+    CU(cudaSetDevice(t->cl->dev[r]));
+    if (next_req) CU(cudaMemcpy((uint8_t*)next_req + a * t->msg, k.d.req, n * t->msg, cudaMemcpyDeviceToHost));
+    if (next_dst) CU(cudaMemcpy(next_dst + a, k.d.dst, n, cudaMemcpyDeviceToHost));
+    if (last_resp) CU(cudaMemcpy((uint8_t*)last_resp + z * t->msg, k.out, k.last_n * t->msg, cudaMemcpyDeviceToHost));
+    a += n;
+    z += k.last_n;
+  }
+  if (n_next) *n_next = a;
+  if (n_last) *n_last = z;
+  return DINT_OK;
+}
+
+// out: rounds timed, their wall time on the host (s), and the CUDA-event time of their device work on rank 0 (s)
+int dint_txn_clients_times(dint_txn_clients* t, double out[3]) {
+  if (!t || !out) return set_err(DINT_EINVAL, "null argument");
+  out[0] = (double)t->timed; out[1] = t->wall_s; out[2] = t->dev_s;
   return DINT_OK;
 }
 

@@ -50,7 +50,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_run", "dint_clients_stats", "dint_clients_peek", "dint_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_run", "dint_clients_stats", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -101,6 +101,12 @@ def lib():
     L.dint_clients_stats.restype = i32; L.dint_clients_stats.argtypes = [vp, C.POINTER(u64)]
     L.dint_clients_peek.restype = i32; L.dint_clients_peek.argtypes = [vp, vp, vp]
     L.dint_clients_destroy.restype = None; L.dint_clients_destroy.argtypes = [vp]
+    L.dint_txn_clients_create.restype = i32; L.dint_txn_clients_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
+    L.dint_txn_clients_run.restype = i32; L.dint_txn_clients_run.argtypes = [vp, u32]
+    L.dint_txn_clients_stats.restype = i32; L.dint_txn_clients_stats.argtypes = [vp, C.POINTER(u64)]
+    L.dint_txn_clients_peek.restype = i32; L.dint_txn_clients_peek.argtypes = [vp, vp, vp, C.POINTER(u64), vp, C.POINTER(u64)]
+    L.dint_txn_clients_times.restype = i32; L.dint_txn_clients_times.argtypes = [vp, C.POINTER(C.c_double)]
+    L.dint_txn_clients_destroy.restype = None; L.dint_txn_clients_destroy.argtypes = [vp]
     L.dint_snapshot_create.restype = i32; L.dint_snapshot_create.argtypes = [vp, C.POINTER(vp)]
     L.dint_snapshot_restore.restype = i32; L.dint_snapshot_restore.argtypes = [vp, vp]
     L.dint_snapshot_destroy.restype = None; L.dint_snapshot_destroy.argtypes = [vp]
@@ -500,6 +506,85 @@ class GpuCluster:
     def close(self):
         if getattr(self, "h", None):
             lib().dint_cluster_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GpuTxnClients:
+    """TATP or SmallBank closed-loop clients resident on the GPUs of `cluster` (a GpuCluster of that kind;
+    dint_txn_clients_*): the state machines of TxnWorkload, draw for draw, with every round emitted on the devices
+    and served by one exchange step.  subscribers: kSubscriberNum (tatp) or kAccountNum (smallbank) of the key
+    generators, as in TxnWorkload -- it must match the servers' population.  Keep the cluster open while these
+    clients exist."""
+
+    def __init__(self, cluster, n_clients, subscribers=None, gid0=0):
+        from .wire import TATP
+        if subscribers is None:
+            subscribers = 7_000_000 if cluster.kind == TATP else 24_000_000
+        self.cluster, self.kind, self.msg, self.n = cluster, cluster.kind, cluster.msg, n_clients
+        h = C.c_void_p()
+        rc = lib().dint_txn_clients_create(cluster.h, n_clients, gid0, subscribers, C.byref(h))
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_create")
+        self.h = h
+
+    def run(self, rounds, check=True):
+        """Serve `rounds` closed-loop rounds; returns when they are served."""
+        rc = lib().dint_txn_clients_run(self.h, rounds)
+        if rc != 0 and (check or rc != DINT_EPROTO):
+            raise DintError(rc, "dint_txn_clients_run")
+        return rc
+
+    def stats(self):
+        """TxnWorkload.stats()'s dict (requests and rounds count what was served) plus fallback_rounds, the rounds
+        served in pieces because they did not fit the cluster's slabs or batch size."""
+        from .txn_workloads import SMALLBANK_TXN_NAMES, TATP_TXN_NAMES
+        from .wire import TATP
+        out = (C.c_uint64 * 19)()
+        rc = lib().dint_txn_clients_stats(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_stats")
+        d = {"requests": int(out[0]), "txns": int(out[1]), "committed": int(out[2]), "rounds": int(out[3])}
+        names = TATP_TXN_NAMES if self.kind == TATP else SMALLBANK_TXN_NAMES
+        d["by_type"] = {n: (int(out[4 + i]), int(out[11 + i])) for i, n in enumerate(names)}
+        d["fallback_rounds"] = int(out[18])
+        return d
+
+    def peek(self):
+        """(next_req, next_dst, last_resp) in global client order: the pending round's requests and destination
+        shards, and the replies the clients absorbed last."""
+        cap = self.n * 9
+        rq = np.empty(cap * self.msg, dtype=np.uint8)
+        dst = np.empty(cap, dtype=np.uint8)
+        rs = np.empty(cap * self.msg, dtype=np.uint8)
+        nn, nl = C.c_uint64(), C.c_uint64()
+        rc = lib().dint_txn_clients_peek(self.h, rq.ctypes.data, dst.ctypes.data, C.byref(nn), rs.ctypes.data, C.byref(nl))
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_peek")
+        return rq[: nn.value * self.msg], dst[: nn.value], rs[: nl.value * self.msg]
+
+    def times(self):
+        """Rounds timed by run(), their host wall time and the CUDA-event time of their device work (rank 0), in s."""
+        out = (C.c_double * 3)()
+        rc = lib().dint_txn_clients_times(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_times")
+        return {"rounds": int(out[0]), "wall_s": out[1], "device_s": out[2]}
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().dint_txn_clients_destroy(self.h)
             self.h = None
 
     def __enter__(self):

@@ -289,6 +289,32 @@ int dint_clients_stats(dint_clients *c, uint64_t out[5]);
 int dint_clients_peek(dint_clients *c, void *next_req_host, void *last_resp_host);
 void dint_clients_destroy(dint_clients *c);
 
+/*
+ * TATP and SmallBank closed-loop clients ON the GPU, against a shard cluster (kind and shard count from the cluster:
+ * tatp or smallbank, 1 or 3-8 shards).  The state machines are those of the host drivers (TxnWorkload,
+ * dint_b200/csrc/txn_clients.cuh is the one statement of both): same draws, same decisions, same records in the same
+ * order.  Clients [gid0, gid0 + n_clients) are split over the cluster's ranks in contiguous blocks; `subscribers` is
+ * kSubscriberNum (tatp) or kAccountNum (smallbank), as in the host drivers, and must match the servers' population.
+ * The cluster must outlive the clients.
+ *   dint_txn_clients_run (blocking): `rounds` rounds, each emitted on the devices and served with one exchange step;
+ *     one host synchronise per round reads the round's per-(rank, shard) record counts, which size the exchange slabs
+ *     exactly.  A round that does not fit the cluster's slabs or batch size is served in pieces (counted in stats[18]).
+ *     Returns 0, DINT_EPROTO (an engine answered with an error reply), or an error.
+ *   dint_txn_clients_stats: dint_txn_stats' 18 words (requests and rounds SERVED), then rounds served in pieces.
+ *   dint_txn_clients_peek (test hook, synchronises): in global client order, the pending round (n_next records and
+ *     their destination shards) and the replies absorbed last (n_last records); buffers of n_clients * 9 records.
+ *   dint_txn_clients_times: rounds timed by run, their host wall time (s) and the CUDA-event time (s) of their device
+ *     work on rank 0's stream; the difference is the host time the round-trip leaves exposed.
+ * The first round is emitted by the first run, peek or stats call.
+ */
+typedef struct dint_txn_clients dint_txn_clients;
+int dint_txn_clients_create(dint_cluster *c, uint32_t n_clients, uint32_t gid0, uint32_t subscribers, dint_txn_clients **out);
+int dint_txn_clients_run(dint_txn_clients *t, uint32_t rounds);
+int dint_txn_clients_stats(dint_txn_clients *t, uint64_t out[19]);
+int dint_txn_clients_peek(dint_txn_clients *t, void *next_req, uint8_t *next_dst, uint64_t *n_next, void *last_resp, uint64_t *n_last);
+int dint_txn_clients_times(dint_txn_clients *t, double out[3]);
+void dint_txn_clients_destroy(dint_txn_clients *t);
+
 int dint_get_stats(dint_engine *e, dint_stats *s);
 void dint_reset_stats(dint_engine *e);
 /* per-kernel CUDA-event timing: 0 = off, 1 = every kernel, otherwise a bit mask over
