@@ -222,6 +222,12 @@ static int launch_chunk_t(dint_engine* e, const Ctx& c, cudaStream_t s) {
     int grid = (int)c.n_tiles < e->grid_apply ? (int)c.n_tiles : e->grid_apply;
     CU(launch_ex(e, k_apply<KIND>, grid, kTile, e->smem_stage, s, false, c));
   }
+  if (KIND == K_TATP && c.n > c.ring_n) {                // (a chunk appends at most n entries: none can be skipped otherwise)
+    int grid = (int)((c.ring_n + kThreads - 1) / kThreads);   // the last ring_n appends end every slot's history
+    if (e->sms > 0 && grid > 4 * e->sms) grid = 4 * e->sms;
+    k_log_vals<<<grid, kThreads, 0, s>>>(c);
+    e->stats.kernel_launches++;
+  }
   if (KIND != K_LOG) {   // the log server has no per-key state: nothing to order
     ProfScope ps(e, s, KT_ORDERED);
     Ctx f = c;           // this chunk's own counters / replies
@@ -693,6 +699,7 @@ static int create_impl(dint_engine* e) {
   if ((rc = dalloc(e, &c.log_tilecnt, e->max_tiles))) return rc;
   if ((rc = dalloc(e, &c.log_tilebase, e->max_tiles))) return rc;
   if ((rc = dalloc(e, &c.log_total, 2))) return rc;
+  if (e->kind == DINT_TATP && (rc = dalloc(e, &c.log_src, ch))) return rc;
   if ((rc = dalloc(e, &c.counters, kNumCounters))) return rc;
   if ((rc = dalloc(e, &c.gbar, 4))) return rc;
 

@@ -151,6 +151,8 @@ struct Ctx {
   uint32_t pad_ok;                // 1 inside the multi-GPU step: type 0xFE records are slab padding (else: invalid)
   uint64_t seg_resp[8];           // reply slab of source s (device address, possibly peer memory)
   const uint32_t* skip;           // multi-GPU step: non-zero = a slab overflowed, serve nothing more (see k_p2p_wait)
+  uint32_t* log_src;              // tatp: [chunk] per append of the chunk, (request index << 1) | is kCommitLog (K2, when
+                                  // the chunk appends more than ring_n), for k_log_vals
 };
 
 // address of tile T's replies (T counted from the start of the batch) when the replies are segmented by source

@@ -373,6 +373,30 @@ __global__ void __launch_bounds__(kThreads) k_log_scan(const Ctx c) {
   }
 }
 
+// K2b (tatp): a kDeleteLog append leaves the value bytes of its ring slot as the slot's last kCommitLog wrote them
+// (tatp/udp/server_shard.cc:196-203).  When a chunk appends more than ring_n entries, K2 writes only the last append to
+// every slot (log_keep), so a kDeleteLog it wrote gets its value bytes here: from the last kCommitLog of this chunk to
+// the same slot, or, when there is none, they are already in the ring.
+__global__ void __launch_bounds__(kThreads) k_log_vals(const Ctx c) {
+  using W = Wire<K_TATP>;
+  if (c.skip && __ldcg(c.skip)) return;
+  const unsigned long long base = c.log_tilebase[0], end = c.log_total[1];
+  if (end - base <= c.ring_n) return;
+  for (unsigned long long ord = end - c.ring_n + blockIdx.x * kThreads + threadIdx.x; ord < end; ord += (unsigned long long)gridDim.x * kThreads) {
+    if (c.log_src[ord - base] & 1u) continue;            // a kCommitLog: K2 wrote the whole entry
+    for (unsigned long long o = ord; o >= base + c.ring_n;) {
+      o -= c.ring_n;
+      const uint32_t s = c.log_src[o - base];
+      if (s & 1u) {
+        const uint8_t* src = c.req + (size_t)(s >> 1) * W::MSG + W::VAL;
+        uint8_t* e = c.ring + (size_t)(ord % c.ring_n) * W::LOGENT + 16;
+        for (int b = 0; b < 40; b++) e[b] = src[b];
+        break;
+      }
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------
 // K2 apply
 // ---------------------------------------------------------------------------------------------------
@@ -445,6 +469,8 @@ __global__ void __launch_bounds__(kTile) k_apply(const Ctx c) {
       if (lg) {
         log_ord = c.log_tilebase[t] + r_log;
         log_keep = log_ord + c.ring_n >= c.log_total[1];   // no later append of this chunk overwrites it
+        if (KIND == K_TATP && c.log_total[1] - c.log_tilebase[0] > c.ring_n)
+          c.log_src[log_ord - c.log_tilebase[0]] = ((first + threadIdx.x) << 1) | (rec[W::TYPE] == 14 ? 1u : 0u);
       }
       if (listed) {
         const uint32_t idx = first + threadIdx.x;
