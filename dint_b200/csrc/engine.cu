@@ -1707,9 +1707,11 @@ uint64_t dint_cluster_overflow_retries(dint_cluster* cl) { return cl ? cl->overf
 }  // extern "C"
 
 extern "C" {
-// ---- lock_fasst closed-loop clients on the GPU (clients.cuh) ------------------------------------------------
+// ---- lock_2pl / lock_fasst / log_server / store closed-loop clients on the GPU (clients.cuh) ------------------
 struct dint_clients {
   dint_engine* e = nullptr;
+  int kind = 0;
+  uint32_t msg = 0;
   ClientCtx cc{};
   uint8_t *req = nullptr, *resp = nullptr;
   double* cdf = nullptr;
@@ -1722,41 +1724,90 @@ void dint_clients_destroy(dint_clients* c) {
   cudaSetDevice(c->e->device);
   cudaDeviceSynchronize();
   cudaFree(c->req); cudaFree(c->resp); cudaFree(c->cdf);
-  cudaFree(c->cc.hdr); cudaFree(c->cc.rng); cudaFree(c->cc.rk); cudaFree(c->cc.rv); cudaFree(c->cc.stats);
+  cudaFree(c->cc.hdr); cudaFree(c->cc.rng); cudaFree(c->cc.lcg); cudaFree(c->cc.rk); cudaFree(c->cc.rv); cudaFree(c->cc.stats);
   delete c;
 }
 
-int dint_clients_create(dint_engine* e, uint32_t n_clients, uint64_t seed, uint32_t n_keys, double zipf_theta, uint32_t read_pct,
-                        dint_clients** out) {
-  if (!e || !out || e->kind != DINT_FASST || n_clients == 0 || n_keys == 0) return set_err(DINT_EINVAL, "lock_fasst engine, n_clients > 0, n_keys > 0");
+int dint_clients_create_cfg(dint_engine* e, const dint_clients_cfg* cfg, dint_clients** out) {
+  if (!e || !cfg || !out) return set_err(DINT_EINVAL, "null argument");
+  const int kind = e->kind;
+  const bool lock = kind == DINT_LOCK2PL || kind == DINT_FASST;
+  if (kind == DINT_TATP || kind == DINT_SMALLBANK)
+    return set_err(DINT_EINVAL, "tatp / smallbank engine: their clients are dint_txn_clients_create's");
+  if (cfg->n_clients == 0) return set_err(DINT_EINVAL, "n_clients must be > 0");
+  if ((lock || (kind == DINT_STORE && cfg->store_hot)) && cfg->n_keys == 0)
+    return set_err(DINT_EINVAL, "n_keys must be > 0 for lock clients and HOT store clients");
+  if (cfg->read_pct > 100) return set_err(DINT_EINVAL, "read_pct must be <= 100");
+  if (cfg->set_pct > 100) return set_err(DINT_EINVAL, "set_pct must be <= 100");
+  if (kind == DINT_STORE && !cfg->store_hot && cfg->store_subscribers == 0)
+    return set_err(DINT_EINVAL, "store_subscribers must be > 0 for REF store clients");
   CU(cudaSetDevice(e->device));
   dint_clients* c = new dint_clients();
   c->e = e;
-  c->seed = seed;
+  c->kind = kind;
+  c->msg = kMsgSize[kind];
+  c->seed = cfg->seed;
   ClientCtx& cc = c->cc;
-  cc.n_clients = n_clients; cc.n_keys = n_keys; cc.read_pct = read_pct;
-  const size_t n = n_clients;
-  if (cudaMalloc(&c->req, n * 9 + 16) != cudaSuccess || cudaMalloc(&c->resp, n * 9 + 16) != cudaSuccess ||
-      cudaMalloc(&cc.hdr, n * 8) != cudaSuccess || cudaMalloc(&cc.rng, n * 8) != cudaSuccess || cudaMalloc(&cc.rk, n * 40) != cudaSuccess ||
-      cudaMalloc(&cc.rv, n * 40) != cudaSuccess || cudaMalloc(&cc.stats, 8 * sizeof(unsigned long long)) != cudaSuccess) {
+  cc.n_clients = cfg->n_clients; cc.n_keys = cfg->n_keys; cc.read_pct = cfg->read_pct;
+  cc.set_pct = cfg->set_pct; cc.subscribers = cfg->store_subscribers; cc.store_hot = kind == DINT_STORE && cfg->store_hot ? 1u : 0u;
+  const size_t n = cfg->n_clients;
+  const bool ref_store = kind == DINT_STORE && !cc.store_hot;
+  bool ok = cudaMalloc(&c->req, n * c->msg + 16) == cudaSuccess && cudaMalloc(&c->resp, n * c->msg + 16) == cudaSuccess &&
+            cudaMalloc(&cc.stats, 8 * sizeof(unsigned long long)) == cudaSuccess;
+  if (ok && !ref_store) ok = cudaMalloc(&cc.rng, n * 8) == cudaSuccess;
+  if (ok && ref_store) ok = cudaMalloc(&cc.lcg, n * 8) == cudaSuccess;
+  if (ok && lock) ok = cudaMalloc(&cc.hdr, n * 8) == cudaSuccess && cudaMalloc(&cc.rk, n * 40) == cudaSuccess;
+  if (ok && kind == DINT_FASST) ok = cudaMalloc(&cc.rv, n * 40) == cudaSuccess && cudaMemset(cc.rv, 0, n * 40) == cudaSuccess;
+  if (ok) ok = cudaMemset(cc.stats, 0, 8 * sizeof(unsigned long long)) == cudaSuccess;
+  if (!ok) {
     cudaError_t ce = cudaGetLastError();
     dint_clients_destroy(c);
     return set_err(DINT_ENOMEM, "client state", ce);
   }
-  CU(cudaMemset(cc.stats, 0, 8 * sizeof(unsigned long long)));
-  CU(cudaMemset(cc.rv, 0, n * 40));
-  if (zipf_theta > 0) {                                  // workloads.cc Zipf::init
+  if (cfg->zipf_theta > 0 && (lock || cc.store_hot)) {  // workloads.cc Zipf::init
+    const uint32_t n_keys = cfg->n_keys;
     std::vector<double> cdf(n_keys);
     double acc = 0;
-    for (uint32_t k = 0; k < n_keys; k++) { acc += 1.0 / std::pow((double)(k + 1), zipf_theta); cdf[k] = acc; }
+    for (uint32_t k = 0; k < n_keys; k++) { acc += 1.0 / std::pow((double)(k + 1), cfg->zipf_theta); cdf[k] = acc; }
     for (auto& v : cdf) v /= acc;
-    CU(cudaMalloc(&c->cdf, (size_t)n_keys * sizeof(double)));
-    CU(cudaMemcpy(c->cdf, cdf.data(), (size_t)n_keys * sizeof(double), cudaMemcpyHostToDevice));
+    if (cudaMalloc(&c->cdf, (size_t)n_keys * sizeof(double)) != cudaSuccess ||
+        cudaMemcpy(c->cdf, cdf.data(), (size_t)n_keys * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaError_t ce = cudaGetLastError();
+      dint_clients_destroy(c);
+      return set_err(DINT_ENOMEM, "Zipf table", ce);
+    }
     cc.cdf = c->cdf;
     cc.zipf_n = n_keys;
   }
   *out = c;
   return DINT_OK;
+}
+
+int dint_clients_create(dint_engine* e, uint32_t n_clients, uint64_t seed, uint32_t n_keys, double zipf_theta, uint32_t read_pct,
+                        dint_clients** out) {
+  if (!e || !out || e->kind != DINT_FASST || n_clients == 0 || n_keys == 0) return set_err(DINT_EINVAL, "lock_fasst engine, n_clients > 0, n_keys > 0");
+  dint_clients_cfg cfg{};
+  cfg.n_clients = n_clients; cfg.n_keys = n_keys; cfg.seed = seed; cfg.zipf_theta = zipf_theta;
+  cfg.read_pct = read_pct < 100 ? read_pct : 100;        // every read_pct >= 100 means "no key is written"
+  return dint_clients_create_cfg(e, &cfg, out);
+}
+
+// one kernel of the clients on s: first = every client starts and emits its first request; otherwise absorb the
+// replies in resp and emit the next round's requests
+static void clients_launch(dint_clients* c, bool first, cudaStream_t s) {
+  const uint32_t blocks = (c->cc.n_clients + 255) / 256;
+  switch (c->kind) {
+    case DINT_FASST:
+      if (first) k_clients_init<K_FASST><<<blocks, 256, 0, s>>>(c->cc, c->seed, c->req);
+      else k_clients_step<K_FASST><<<blocks, 256, 0, s>>>(c->cc, c->resp, c->req);
+      break;
+    case DINT_LOCK2PL:
+      if (first) k_clients_init<K_LOCK2PL><<<blocks, 256, 0, s>>>(c->cc, c->seed, c->req);
+      else k_clients_step<K_LOCK2PL><<<blocks, 256, 0, s>>>(c->cc, c->resp, c->req);
+      break;
+    case DINT_LOG: k_log_clients<<<blocks, 256, 0, s>>>(c->cc, c->seed, first ? 1u : 0u, c->req); break;
+    default: k_store_clients<<<blocks, 256, 0, s>>>(c->cc, c->seed, first ? 1u : 0u, c->resp, c->req); break;
+  }
 }
 
 // `rounds` closed-loop rounds, asynchronous on cuda_stream: every round = the engine on the clients' request buffer
@@ -1766,16 +1817,15 @@ int dint_clients_run(dint_clients* c, uint32_t rounds, void* cuda_stream) {
   dint_engine* e = c->e;
   CU(cudaSetDevice(e->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;
-  const uint32_t blocks = (c->cc.n_clients + 255) / 256;
   if (!c->started) {
-    k_clients_init<<<blocks, 256, 0, s>>>(c->cc, c->seed, c->req);
+    clients_launch(c, true, s);
     c->started = true;
     e->stats.kernel_launches++;
   }
   for (uint32_t r = 0; r < rounds; r++) {
     int rc = run_device(e, c->req, c->cc.n_clients, c->resp, s);
     if (rc) return rc;
-    k_clients_step<<<blocks, 256, 0, s>>>(c->cc, c->resp, c->req);
+    clients_launch(c, false, s);
     e->stats.kernel_launches++;
   }
   CU(cudaGetLastError());
@@ -1793,18 +1843,32 @@ int dint_clients_stats(dint_clients* c, uint64_t out[5]) {
   return DINT_OK;
 }
 
-// test hook: the requests the clients will send next and the replies they absorbed last (host buffers of n_clients * 9 bytes)
+// out: requests served, committed transactions, validation aborts, lock rejects, not-exist replies, rounds (the order of
+// dint_wl_stats; synchronises)
+int dint_clients_stats_all(dint_clients* c, uint64_t out[6]) {
+  if (!c || !out) return set_err(DINT_EINVAL, "null argument");
+  CU(cudaSetDevice(c->e->device));
+  CU(cudaDeviceSynchronize());
+  unsigned long long h[6];
+  CU(cudaMemcpy(h, c->cc.stats, sizeof h, cudaMemcpyDeviceToHost));
+  out[0] = h[0]; out[1] = h[1]; out[2] = h[2]; out[3] = h[3]; out[4] = h[5]; out[5] = h[4];
+  return DINT_OK;
+}
+
+// test hook: the requests the clients will send next and the replies they absorbed last (host buffers of
+// n_clients * dint_msg_size(kind) bytes)
 int dint_clients_peek(dint_clients* c, void* next_req_host, void* last_resp_host) {
   if (!c) return set_err(DINT_EINVAL, "null argument");
   CU(cudaSetDevice(c->e->device));
   CU(cudaDeviceSynchronize());
   if (!c->started) {
-    k_clients_init<<<(c->cc.n_clients + 255) / 256, 256>>>(c->cc, c->seed, c->req);
+    clients_launch(c, true, 0);
     c->started = true;
     CU(cudaDeviceSynchronize());
   }
-  if (next_req_host) CU(cudaMemcpy(next_req_host, c->req, (size_t)c->cc.n_clients * 9, cudaMemcpyDeviceToHost));
-  if (last_resp_host) CU(cudaMemcpy(last_resp_host, c->resp, (size_t)c->cc.n_clients * 9, cudaMemcpyDeviceToHost));
+  const size_t bytes = (size_t)c->cc.n_clients * c->msg;
+  if (next_req_host) CU(cudaMemcpy(next_req_host, c->req, bytes, cudaMemcpyDeviceToHost));
+  if (last_resp_host) CU(cudaMemcpy(last_resp_host, c->resp, bytes, cudaMemcpyDeviceToHost));
   return DINT_OK;
 }
 

@@ -41,6 +41,12 @@ class DintPeerPtrs(C.Structure):
         return o
 
 
+class DintClientsCfg(C.Structure):
+    _fields_ = [("n_clients", C.c_uint32), ("n_keys", C.c_uint32), ("seed", C.c_uint64), ("zipf_theta", C.c_double),
+                ("read_pct", C.c_uint32), ("set_pct", C.c_uint32), ("store_subscribers", C.c_uint32),
+                ("store_hot", C.c_uint32), ("reserved", C.c_uint32 * 4)]
+
+
 class DintKernelTime(C.Structure):
     _fields_ = [("name", C.c_char * 32), ("launches", C.c_uint64), ("total_ms", C.c_double)]
 
@@ -50,7 +56,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_run", "dint_clients_stats", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -97,8 +103,10 @@ def lib():
     L.dint_shard_recover.restype = i32; L.dint_shard_recover.argtypes = [vp, u32, C.POINTER(u32)]
     L.dint_cluster_destroy.restype = None; L.dint_cluster_destroy.argtypes = [vp]
     L.dint_clients_create.restype = i32; L.dint_clients_create.argtypes = [vp, u32, u64, u32, C.c_double, u32, C.POINTER(vp)]
+    L.dint_clients_create_cfg.restype = i32; L.dint_clients_create_cfg.argtypes = [vp, C.POINTER(DintClientsCfg), C.POINTER(vp)]
     L.dint_clients_run.restype = i32; L.dint_clients_run.argtypes = [vp, u32, vp]
     L.dint_clients_stats.restype = i32; L.dint_clients_stats.argtypes = [vp, C.POINTER(u64)]
+    L.dint_clients_stats_all.restype = i32; L.dint_clients_stats_all.argtypes = [vp, C.POINTER(u64)]
     L.dint_clients_peek.restype = i32; L.dint_clients_peek.argtypes = [vp, vp, vp]
     L.dint_clients_destroy.restype = None; L.dint_clients_destroy.argtypes = [vp]
     L.dint_txn_clients_create.restype = i32; L.dint_txn_clients_create.argtypes = [vp, u32, u32, u32, C.POINTER(vp)]
@@ -418,14 +426,20 @@ class Engine:
 
 
 class GpuClients:
-    """lock_fasst closed-loop clients resident on the GPU next to `engine` (dint_clients_*)."""
+    """Closed-loop clients resident on the GPU next to `engine` (dint_clients_*), of the engine's kind: lock_2pl,
+    lock_fasst, log_server or store.  The keyword arguments are those of workloads.Workload, so one dict of them
+    drives the GPU clients and the host clients alike."""
 
-    def __init__(self, engine, n_clients, seed=20230, n_keys=24_000_000, zipf_theta=0.0, read_pct=80):
-        self.engine, self.n = engine, n_clients
+    def __init__(self, engine, n_clients, seed=20230, n_keys=24_000_000, zipf_theta=0.0, read_pct=80, set_pct=0,
+                 store_subscribers=2_000_000, store_hot=False):
+        self.engine, self.n, self.kind = engine, n_clients, engine.kind
+        self.msg = MSG_SIZE[self.kind]
+        cfg = DintClientsCfg(n_clients=n_clients, n_keys=n_keys, seed=seed, zipf_theta=zipf_theta, read_pct=read_pct,
+                             set_pct=set_pct, store_subscribers=store_subscribers, store_hot=1 if store_hot else 0)
         h = C.c_void_p()
-        rc = lib().dint_clients_create(engine.h, n_clients, seed, n_keys, zipf_theta, read_pct, C.byref(h))
+        rc = lib().dint_clients_create_cfg(engine.h, C.byref(cfg), C.byref(h))
         if rc != 0:
-            raise DintError(rc, "dint_clients_create")
+            raise DintError(rc, "dint_clients_create_cfg")
         self.h = h
 
     def run(self, rounds, stream=None):
@@ -437,15 +451,18 @@ class GpuClients:
             raise DintError(rc, "dint_clients_run")
 
     def stats(self):
-        out = (C.c_uint64 * 5)()
-        rc = lib().dint_clients_stats(self.h, out)
+        """the counters of workloads.Workload.stats(), under the same keys"""
+        out = (C.c_uint64 * 6)()
+        rc = lib().dint_clients_stats_all(self.h, out)
         if rc != 0:
-            raise DintError(rc, "dint_clients_stats")
-        return dict(zip(["requests", "committed", "validation_aborts", "lock_rejects", "rounds"], [int(x) for x in out]))
+            raise DintError(rc, "dint_clients_stats_all")
+        keys = ["requests", "committed", "validation_aborts", "lock_rejects", "not_exist", "rounds"]
+        return dict(zip(keys, [int(x) for x in out]))
 
     def peek(self):
-        rq = np.empty(self.n * 9, dtype=np.uint8)
-        rs = np.empty(self.n * 9, dtype=np.uint8)
+        """(the requests the clients send next, the replies they absorbed last): uint8 arrays of n_clients * msg bytes"""
+        rq = np.empty(self.n * self.msg, dtype=np.uint8)
+        rs = np.empty(self.n * self.msg, dtype=np.uint8)
         rc = lib().dint_clients_peek(self.h, rq.ctypes.data, rs.ctypes.data)
         if rc != 0:
             raise DintError(rc, "dint_clients_peek")
@@ -455,6 +472,12 @@ class GpuClients:
         if getattr(self, "h", None):
             lib().dint_clients_destroy(self.h)
             self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
 
     def __del__(self):
         try:
