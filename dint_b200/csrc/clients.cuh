@@ -19,9 +19,12 @@
 //   rk[i][c]  u32  read set, ascending (i < nr)          rv[i][c]  u32  version read for rk[i] (lock_fasst only)
 // store / log_server (k_store_clients / k_log_clients): one request is one transaction; the only state is the draw
 // stream (rng[c], or the reference's LCG lcg[c] for the REF store family).
+// Against a shard cluster (dint_cluster_clients_*) each rank holds a contiguous block of the clients, offset by id0, and
+// k_clients_owner_count tells the host how many of the rank's records each shard owns before the round is exchanged.
 #pragma once
 #include "common.cuh"
 #include "engine.cuh"
+#include "kernels.cuh"
 
 namespace dint {
 
@@ -31,6 +34,8 @@ enum : uint32_t { CPH_READ = 0, CPH_ACQ, CPH_VALIDATE, CPH_ABORT, CPH_COMMIT, CP
 struct ClientCtx {
   uint32_t n_clients, n_keys, read_pct, zipf_n;     // zipf_n != 0: keys are Zipf ranks, cdf[zipf_n]
   uint32_t set_pct, subscribers, store_hot;         // store: percent of kSet, kSubscriberNum, HOT family
+  uint32_t id0;                                     // global id of client 0 of this block (0 on one engine; a cluster
+                                                    // rank's first client): seeds the draw streams, never indexes state
   const double* cdf;
   unsigned long long* hdr;                          // lock kinds
   unsigned long long* rng;                          // lock kinds, log_server, HOT store
@@ -144,7 +149,7 @@ template <int KIND>
 __global__ void __launch_bounds__(256) k_clients_init(const ClientCtx c, unsigned long long seed, uint8_t* req) {
   const uint32_t id = blockIdx.x * blockDim.x + threadIdx.x;
   if (id >= c.n_clients) return;
-  CRng r = client_rng(seed, id);
+  CRng r = client_rng(seed, c.id0 + id);
   client_start_txn<KIND>(c, id, r, req);
   c.rng[id] = r.s;
 }
@@ -298,14 +303,14 @@ __global__ void __launch_bounds__(256) k_store_clients(const ClientCtx c, unsign
     bool is_set;
     uint32_t s_id, sf, st, end_time = 0;
     if (c.store_hot) {                              // HOT: the first n_keys of the population, xorshift + Zipf
-      CRng r = first ? client_rng(seed, id) : CRng{c.rng[id]};
+      CRng r = first ? client_rng(seed, c.id0 + id) : CRng{c.rng[id]};
       is_set = r.below(100) < c.set_pct;
       const uint32_t k = client_draw_key(c, r);
       s_id = k / 12; sf = (k % 12) / 3 + 1; st = (k % 3) * 8;
       end_time = r.below(24);
       c.rng[id] = r.s;
     } else {                                        // REF: lcg = 0xdeadbeef + client index (client_udp.cc:201)
-      unsigned long long l = first ? 0xdeadbeefULL + id : c.lcg[id];
+      unsigned long long l = first ? 0xdeadbeefULL + c.id0 + id : c.lcg[id];
       is_set = store_fastrand(l) % 100 >= 100 - c.set_pct;   // workgen_arr: reads first, sets last
       const uint32_t x = store_fastrand(l), y = store_fastrand(l);
       s_id = ((x % c.subscribers) | (y & 1048575u)) % c.subscribers;   // NURand
@@ -336,7 +341,7 @@ __global__ void __launch_bounds__(256) k_log_clients(const ClientCtx c, unsigned
   __shared__ __align__(16) uint8_t s_rec[kKvSlice];
   const uint32_t id = blockIdx.x * blockDim.x + threadIdx.x;
   if (id < c.n_clients) {
-    CRng r = first ? client_rng(seed, id) : CRng{c.rng[id]};
+    CRng r = first ? client_rng(seed, c.id0 + id) : CRng{c.rng[id]};
     uint32_t p[13];
     p[0] = r.below(7010000); p[1] = 0;
 #pragma unroll
@@ -352,6 +357,37 @@ __global__ void __launch_bounds__(256) k_log_clients(const ClientCtx c, unsigned
     atomicAdd(&c.stats[1], (unsigned long long)c.n_clients);
     atomicAdd(&c.stats[4], 1ULL);
   }
+}
+
+// ---- a cluster rank's round, counted per owner shard (dint_cluster_clients_*) ----------------------------------------
+// route_owner_of is what k_route_dispatch computes, so the counts are exact.  Every CTA adds its counts to acc[0, 8); the
+// last CTA to finish (ticket acc[8]) publishes them to the mapped pinned block pub -- [0] records, [1 + o] records for
+// shard o, the layout of the txn clients' -- and resets acc for the next round.
+template <int KIND>
+__global__ void __launch_bounds__(kThreads) k_clients_owner_count(const Ctx c, const uint8_t* req, uint32_t n, uint32_t* acc,
+                                                                  uint32_t* pub) {
+  __shared__ uint32_t s_cnt[kMaxShards];
+  __shared__ bool s_last;
+  if (threadIdx.x < kMaxShards) s_cnt[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t i = blockIdx.x * kThreads + threadIdx.x;
+  const uint32_t o = i < n ? route_owner_of<KIND>(c, req + (size_t)i * Wire<KIND>::MSG) : 0xffu;
+  const uint32_t peers = __match_any_sync(0xffffffffu, o);
+  if (o < kMaxShards && (int)lane_id() == __ffs(peers) - 1) atomicAdd(&s_cnt[o], (uint32_t)__popc(peers));
+  __syncthreads();
+  if (threadIdx.x < kMaxShards && s_cnt[threadIdx.x]) atomicAdd(&acc[threadIdx.x], s_cnt[threadIdx.x]);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(&acc[kMaxShards], 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  if (threadIdx.x == 0) pub[0] = n;
+  if (threadIdx.x < kMaxShards) {
+    pub[1 + threadIdx.x] = ((volatile uint32_t*)acc)[threadIdx.x];
+    acc[threadIdx.x] = 0;
+  }
+  if (threadIdx.x == 0) acc[kMaxShards] = 0;
 }
 #endif  // __CUDACC__
 

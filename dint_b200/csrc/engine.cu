@@ -1706,34 +1706,27 @@ uint64_t dint_cluster_overflow_retries(dint_cluster* cl) { return cl ? cl->overf
 
 }  // extern "C"
 
-extern "C" {
 // ---- lock_2pl / lock_fasst / log_server / store closed-loop clients on the GPU (clients.cuh) ------------------
-struct dint_clients {
-  dint_engine* e = nullptr;
-  int kind = 0;
-  uint32_t msg = 0;
+// One block of clients on one device: their state, the requests of the pending round and the replies they absorb next.
+// dint_clients holds one next to its engine; dint_cluster_clients holds one per cluster rank.
+struct ClientBlock {
   ClientCtx cc{};
   uint8_t *req = nullptr, *resp = nullptr;
   double* cdf = nullptr;
-  uint64_t seed = 0;
-  bool started = false;
 };
 
-void dint_clients_destroy(dint_clients* c) {
-  if (!c) return;
-  cudaSetDevice(c->e->device);
-  cudaDeviceSynchronize();
-  cudaFree(c->req); cudaFree(c->resp); cudaFree(c->cdf);
-  cudaFree(c->cc.hdr); cudaFree(c->cc.rng); cudaFree(c->cc.lcg); cudaFree(c->cc.rk); cudaFree(c->cc.rv); cudaFree(c->cc.stats);
-  delete c;
+static void client_block_free(ClientBlock& b) {
+  cudaFree(b.req); cudaFree(b.resp); cudaFree(b.cdf);
+  cudaFree(b.cc.hdr); cudaFree(b.cc.rng); cudaFree(b.cc.lcg); cudaFree(b.cc.rk); cudaFree(b.cc.rv); cudaFree(b.cc.stats);
+  b = ClientBlock{};
 }
 
-int dint_clients_create_cfg(dint_engine* e, const dint_clients_cfg* cfg, dint_clients** out) {
-  if (!e || !cfg || !out) return set_err(DINT_EINVAL, "null argument");
-  const int kind = e->kind;
+// The argument checks of every lock / store / log client handle, then the state of clients [id0, id0 + n) of the family
+// `cfg` on `device` (n may be 0: a cluster rank without clients).  On an error nothing stays allocated.
+static int client_block_make(int kind, const dint_clients_cfg* cfg, int device, uint32_t id0, uint32_t n, ClientBlock* out) {
   const bool lock = kind == DINT_LOCK2PL || kind == DINT_FASST;
   if (kind == DINT_TATP || kind == DINT_SMALLBANK)
-    return set_err(DINT_EINVAL, "tatp / smallbank engine: their clients are dint_txn_clients_create's");
+    return set_err(DINT_EINVAL, "tatp / smallbank: their clients are dint_txn_clients_*");
   if (cfg->n_clients == 0) return set_err(DINT_EINVAL, "n_clients must be > 0");
   if ((lock || (kind == DINT_STORE && cfg->store_hot)) && cfg->n_keys == 0)
     return set_err(DINT_EINVAL, "n_keys must be > 0 for lock clients and HOT store clients");
@@ -1741,27 +1734,24 @@ int dint_clients_create_cfg(dint_engine* e, const dint_clients_cfg* cfg, dint_cl
   if (cfg->set_pct > 100) return set_err(DINT_EINVAL, "set_pct must be <= 100");
   if (kind == DINT_STORE && !cfg->store_hot && cfg->store_subscribers == 0)
     return set_err(DINT_EINVAL, "store_subscribers must be > 0 for REF store clients");
-  CU(cudaSetDevice(e->device));
-  dint_clients* c = new dint_clients();
-  c->e = e;
-  c->kind = kind;
-  c->msg = kMsgSize[kind];
-  c->seed = cfg->seed;
-  ClientCtx& cc = c->cc;
-  cc.n_clients = cfg->n_clients; cc.n_keys = cfg->n_keys; cc.read_pct = cfg->read_pct;
+  CU(cudaSetDevice(device));
+  ClientBlock b;
+  ClientCtx& cc = b.cc;
+  const uint32_t msg = kMsgSize[kind];
+  cc.n_clients = n; cc.id0 = id0; cc.n_keys = cfg->n_keys; cc.read_pct = cfg->read_pct;
   cc.set_pct = cfg->set_pct; cc.subscribers = cfg->store_subscribers; cc.store_hot = kind == DINT_STORE && cfg->store_hot ? 1u : 0u;
-  const size_t n = cfg->n_clients;
+  const size_t na = n ? n : 1;                          // an empty block still gets valid pointers
   const bool ref_store = kind == DINT_STORE && !cc.store_hot;
-  bool ok = cudaMalloc(&c->req, n * c->msg + 16) == cudaSuccess && cudaMalloc(&c->resp, n * c->msg + 16) == cudaSuccess &&
+  bool ok = cudaMalloc(&b.req, na * msg + 16) == cudaSuccess && cudaMalloc(&b.resp, na * msg + 16) == cudaSuccess &&
             cudaMalloc(&cc.stats, 8 * sizeof(unsigned long long)) == cudaSuccess;
-  if (ok && !ref_store) ok = cudaMalloc(&cc.rng, n * 8) == cudaSuccess;
-  if (ok && ref_store) ok = cudaMalloc(&cc.lcg, n * 8) == cudaSuccess;
-  if (ok && lock) ok = cudaMalloc(&cc.hdr, n * 8) == cudaSuccess && cudaMalloc(&cc.rk, n * 40) == cudaSuccess;
-  if (ok && kind == DINT_FASST) ok = cudaMalloc(&cc.rv, n * 40) == cudaSuccess && cudaMemset(cc.rv, 0, n * 40) == cudaSuccess;
+  if (ok && !ref_store) ok = cudaMalloc(&cc.rng, na * 8) == cudaSuccess;
+  if (ok && ref_store) ok = cudaMalloc(&cc.lcg, na * 8) == cudaSuccess;
+  if (ok && lock) ok = cudaMalloc(&cc.hdr, na * 8) == cudaSuccess && cudaMalloc(&cc.rk, na * 40) == cudaSuccess;
+  if (ok && kind == DINT_FASST) ok = cudaMalloc(&cc.rv, na * 40) == cudaSuccess && cudaMemset(cc.rv, 0, na * 40) == cudaSuccess;
   if (ok) ok = cudaMemset(cc.stats, 0, 8 * sizeof(unsigned long long)) == cudaSuccess;
   if (!ok) {
     cudaError_t ce = cudaGetLastError();
-    dint_clients_destroy(c);
+    client_block_free(b);
     return set_err(DINT_ENOMEM, "client state", ce);
   }
   if (cfg->zipf_theta > 0 && (lock || cc.store_hot)) {  // workloads.cc Zipf::init
@@ -1770,15 +1760,67 @@ int dint_clients_create_cfg(dint_engine* e, const dint_clients_cfg* cfg, dint_cl
     double acc = 0;
     for (uint32_t k = 0; k < n_keys; k++) { acc += 1.0 / std::pow((double)(k + 1), cfg->zipf_theta); cdf[k] = acc; }
     for (auto& v : cdf) v /= acc;
-    if (cudaMalloc(&c->cdf, (size_t)n_keys * sizeof(double)) != cudaSuccess ||
-        cudaMemcpy(c->cdf, cdf.data(), (size_t)n_keys * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (cudaMalloc(&b.cdf, (size_t)n_keys * sizeof(double)) != cudaSuccess ||
+        cudaMemcpy(b.cdf, cdf.data(), (size_t)n_keys * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
       cudaError_t ce = cudaGetLastError();
-      dint_clients_destroy(c);
+      client_block_free(b);
       return set_err(DINT_ENOMEM, "Zipf table", ce);
     }
-    cc.cdf = c->cdf;
+    cc.cdf = b.cdf;
     cc.zipf_n = n_keys;
   }
+  *out = b;
+  return DINT_OK;
+}
+
+// one kernel of a block of clients on s: first = every client starts and emits its first request; otherwise absorb the
+// replies in resp and emit the next round's requests
+static void clients_launch(int kind, uint64_t seed, const ClientBlock& b, bool first, cudaStream_t s) {
+  const uint32_t blocks = (b.cc.n_clients + 255) / 256;
+  if (!blocks) return;
+  switch (kind) {
+    case DINT_FASST:
+      if (first) k_clients_init<K_FASST><<<blocks, 256, 0, s>>>(b.cc, seed, b.req);
+      else k_clients_step<K_FASST><<<blocks, 256, 0, s>>>(b.cc, b.resp, b.req);
+      break;
+    case DINT_LOCK2PL:
+      if (first) k_clients_init<K_LOCK2PL><<<blocks, 256, 0, s>>>(b.cc, seed, b.req);
+      else k_clients_step<K_LOCK2PL><<<blocks, 256, 0, s>>>(b.cc, b.resp, b.req);
+      break;
+    case DINT_LOG: k_log_clients<<<blocks, 256, 0, s>>>(b.cc, seed, first ? 1u : 0u, b.req); break;
+    default: k_store_clients<<<blocks, 256, 0, s>>>(b.cc, seed, first ? 1u : 0u, b.resp, b.req); break;
+  }
+}
+
+extern "C" {
+struct dint_clients {
+  dint_engine* e = nullptr;
+  int kind = 0;
+  uint32_t msg = 0;
+  ClientBlock b;
+  uint64_t seed = 0;
+  bool started = false;
+};
+
+void dint_clients_destroy(dint_clients* c) {
+  if (!c) return;
+  cudaSetDevice(c->e->device);
+  cudaDeviceSynchronize();
+  client_block_free(c->b);
+  delete c;
+}
+
+int dint_clients_create_cfg(dint_engine* e, const dint_clients_cfg* cfg, dint_clients** out) {
+  if (!e || !cfg || !out) return set_err(DINT_EINVAL, "null argument");
+  ClientBlock b;
+  int rc = client_block_make(e->kind, cfg, e->device, 0, cfg->n_clients, &b);
+  if (rc) return rc;
+  dint_clients* c = new dint_clients();
+  c->e = e;
+  c->kind = e->kind;
+  c->msg = kMsgSize[e->kind];
+  c->seed = cfg->seed;
+  c->b = b;
   *out = c;
   return DINT_OK;
 }
@@ -1792,24 +1834,6 @@ int dint_clients_create(dint_engine* e, uint32_t n_clients, uint64_t seed, uint3
   return dint_clients_create_cfg(e, &cfg, out);
 }
 
-// one kernel of the clients on s: first = every client starts and emits its first request; otherwise absorb the
-// replies in resp and emit the next round's requests
-static void clients_launch(dint_clients* c, bool first, cudaStream_t s) {
-  const uint32_t blocks = (c->cc.n_clients + 255) / 256;
-  switch (c->kind) {
-    case DINT_FASST:
-      if (first) k_clients_init<K_FASST><<<blocks, 256, 0, s>>>(c->cc, c->seed, c->req);
-      else k_clients_step<K_FASST><<<blocks, 256, 0, s>>>(c->cc, c->resp, c->req);
-      break;
-    case DINT_LOCK2PL:
-      if (first) k_clients_init<K_LOCK2PL><<<blocks, 256, 0, s>>>(c->cc, c->seed, c->req);
-      else k_clients_step<K_LOCK2PL><<<blocks, 256, 0, s>>>(c->cc, c->resp, c->req);
-      break;
-    case DINT_LOG: k_log_clients<<<blocks, 256, 0, s>>>(c->cc, c->seed, first ? 1u : 0u, c->req); break;
-    default: k_store_clients<<<blocks, 256, 0, s>>>(c->cc, c->seed, first ? 1u : 0u, c->resp, c->req); break;
-  }
-}
-
 // `rounds` closed-loop rounds, asynchronous on cuda_stream: every round = the engine on the clients' request buffer
 // (dint_submit_device) + ONE kernel that absorbs the replies and emits the next round's requests
 int dint_clients_run(dint_clients* c, uint32_t rounds, void* cuda_stream) {
@@ -1818,14 +1842,14 @@ int dint_clients_run(dint_clients* c, uint32_t rounds, void* cuda_stream) {
   CU(cudaSetDevice(e->device));
   cudaStream_t s = (cudaStream_t)cuda_stream;
   if (!c->started) {
-    clients_launch(c, true, s);
+    clients_launch(c->kind, c->seed, c->b, true, s);
     c->started = true;
     e->stats.kernel_launches++;
   }
   for (uint32_t r = 0; r < rounds; r++) {
-    int rc = run_device(e, c->req, c->cc.n_clients, c->resp, s);
+    int rc = run_device(e, c->b.req, c->b.cc.n_clients, c->b.resp, s);
     if (rc) return rc;
-    clients_launch(c, false, s);
+    clients_launch(c->kind, c->seed, c->b, false, s);
     e->stats.kernel_launches++;
   }
   CU(cudaGetLastError());
@@ -1838,7 +1862,7 @@ int dint_clients_stats(dint_clients* c, uint64_t out[5]) {
   CU(cudaSetDevice(c->e->device));
   CU(cudaDeviceSynchronize());
   unsigned long long h[5];
-  CU(cudaMemcpy(h, c->cc.stats, sizeof h, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(h, c->b.cc.stats, sizeof h, cudaMemcpyDeviceToHost));
   for (int i = 0; i < 5; i++) out[i] = h[i];
   return DINT_OK;
 }
@@ -1850,7 +1874,7 @@ int dint_clients_stats_all(dint_clients* c, uint64_t out[6]) {
   CU(cudaSetDevice(c->e->device));
   CU(cudaDeviceSynchronize());
   unsigned long long h[6];
-  CU(cudaMemcpy(h, c->cc.stats, sizeof h, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(h, c->b.cc.stats, sizeof h, cudaMemcpyDeviceToHost));
   out[0] = h[0]; out[1] = h[1]; out[2] = h[2]; out[3] = h[3]; out[4] = h[5]; out[5] = h[4];
   return DINT_OK;
 }
@@ -1862,44 +1886,167 @@ int dint_clients_peek(dint_clients* c, void* next_req_host, void* last_resp_host
   CU(cudaSetDevice(c->e->device));
   CU(cudaDeviceSynchronize());
   if (!c->started) {
-    clients_launch(c, true, 0);
+    clients_launch(c->kind, c->seed, c->b, true, 0);
     c->started = true;
     CU(cudaDeviceSynchronize());
   }
-  const size_t bytes = (size_t)c->cc.n_clients * c->msg;
-  if (next_req_host) CU(cudaMemcpy(next_req_host, c->req, bytes, cudaMemcpyDeviceToHost));
-  if (last_resp_host) CU(cudaMemcpy(last_resp_host, c->resp, bytes, cudaMemcpyDeviceToHost));
+  const size_t bytes = (size_t)c->b.cc.n_clients * c->msg;
+  if (next_req_host) CU(cudaMemcpy(next_req_host, c->b.req, bytes, cudaMemcpyDeviceToHost));
+  if (last_resp_host) CU(cudaMemcpy(last_resp_host, c->b.resp, bytes, cudaMemcpyDeviceToHost));
   return DINT_OK;
 }
 
 }  // extern "C"
 
-extern "C" {
-// ---- TATP / SmallBank closed-loop clients on the GPU against a shard cluster (txn_clients.cuh) ---------------
-// The clients are split over the cluster's ranks in contiguous blocks of gids, rank r's block on rank r's device, so
-// rank-major order is global client order and every shard sees its records in the order one host TxnWorkload would
-// send them.  A round: the step / scan / compact kernels leave the round in req[] / dst[] on every rank and its size
-// and per-shard counts in a pinned block; ONE event synchronise per rank hands those G x (G + 1) words to the host,
-// which sizes the exchange slabs exactly from them and serves the round with one shard_run on device buffers; the
-// clients' next step absorbs the replies straight from out[].  No record crosses PCIe.
-struct TxnRank {
-  txn::DevClients d{};
-  uint32_t tiles = 0;
+// ---- closed-loop clients on the GPU against a shard cluster: the round loop of dint_txn_clients_* and ---------------
+// ---- dint_cluster_clients_* ------------------------------------------------------------------------------------------
+// The clients are split over the cluster's ranks in contiguous blocks, rank r's block on rank r's device, so rank-major
+// order is global client order.  A round: every rank's kernels leave the round in its req[] (and, for client-chosen
+// placements, dst[]) and its size and per-shard counts in a mapped pinned block; ONE event synchronise per rank hands
+// those G x (G + 1) words to the host, which sizes the exchange slabs exactly from them and serves the round with one
+// shard_run on device buffers; the clients' next emission absorbs the replies straight from out[].  No record crosses
+// PCIe.  Serving K rounds without a host round trip is not done: a closed-loop round needs the previous round's replies,
+// and exact slabs need the counts on the host.
+struct RoundRank {
+  const uint8_t* req = nullptr;  // the pending round, contiguous (device)
+  const uint8_t* dst = nullptr;  // its records' owner shards, or null: computed on the device (route_owner_of)
   uint8_t* out = nullptr;        // replies of the round, in the order of req[]
-  uint32_t* pub = nullptr;       // host view of d.pub: [0] records, [1 + o] records for shard o, [9..10] exchange flags
+  uint32_t* pub = nullptr;       // host view of the pinned block: [0] records, [1 + o] records for shard o, [9..10] exchange flags
   cudaEvent_t ev = nullptr;      // this rank's emission of the pending round is done
   uint64_t last_n = 0;           // records of the last round served
 };
-struct dint_txn_clients {
+struct RoundLoop {
   dint_cluster* cl = nullptr;
-  uint32_t msg = 0, n = 0;
-  std::vector<TxnRank> rk;
+  uint32_t msg = 0;
+  bool local = false;            // every rank serves its own batch on its own engine, without the exchange (log_server)
   std::vector<cudaStream_t> mains;
   bool started = false;
   uint64_t requests = 0, rounds = 0, fallback_rounds = 0;
   cudaEvent_t t_beg = nullptr, t_end = nullptr;   // on rank 0's stream: the device work of one round
   uint64_t timed = 0;
   double wall_s = 0, dev_s = 0;
+};
+
+// records of one fallback piece: at most min(cap, max_n), a multiple of 16 so that every device batch stays 16-byte aligned
+static uint32_t fallback_piece(const dint_cluster* cl) { return (uint32_t)((cl->cap < cl->max_n ? cl->cap : cl->max_n) & ~15ull); }
+
+// wait for every rank's pending emission; the exchange flags of the round before it must read zero
+template <class Rank>
+static int round_wait(RoundLoop& L, std::vector<Rank>& rk) {
+  for (uint32_t r = 0; r < L.cl->G; r++) {
+    CU(cudaSetDevice(L.cl->dev[r]));
+    CU(cudaEventSynchronize(rk[r].ev));
+  }
+  for (uint32_t r = 0; r < L.cl->G; r++)
+    if (rk[r].pub[9] || rk[r].pub[10]) return set_err(DINT_EIO, "internal: an exchange slab overflowed or a wait timed out");
+  return DINT_OK;
+}
+static int round_errors(dint_cluster* cl, unsigned long long* sum) {
+  *sum = 0;
+  for (auto* e : cl->eng) {
+    CU(cudaSetDevice(e->device));
+    int rc = pull_counters(e);
+    if (rc) return rc;
+    *sum += e->stats.errors;
+  }
+  return DINT_OK;
+}
+
+// `rounds` rounds, blocking.  emit(first) enqueues one emission on every rank and records each rank's event.
+template <class Rank, class Emit>
+static int serve_rounds(RoundLoop& L, std::vector<Rank>& rk, uint32_t rounds, Emit&& emit) {
+  dint_cluster* cl = L.cl;
+  const uint32_t G = cl->G, msg = L.msg;
+  unsigned long long err_before = 0, err_after = 0;
+  int rc = round_errors(cl, &err_before);
+  if (rc) return rc;
+  if (!L.started && (rc = emit(1))) return rc;
+  if ((rc = round_wait(L, rk))) return rc;
+  const uint32_t piece = fallback_piece(cl);
+  auto round_up = [](uint64_t x) { return (uint32_t)(x ? (x + kTile - 1) / kTile * kTile : kTile); };
+  std::vector<uint64_t> n(G);
+  std::vector<std::vector<ShardBatch>> b;
+  auto t_prev = std::chrono::steady_clock::now();
+  for (uint32_t i = 0; i < rounds; i++) {
+    // the slab capacity of the round: the largest (source, owner) count, so no slab can overflow
+    uint64_t maxc = 0;
+    bool fits = true;
+    for (uint32_t r = 0; r < G; r++) {
+      n[r] = rk[r].pub[0];
+      if (n[r] > cl->max_n) fits = false;
+      for (uint32_t o = 0; o < G; o++) maxc = rk[r].pub[1 + o] > maxc ? rk[r].pub[1 + o] : maxc;
+    }
+    if (maxc > cl->cap) fits = false;
+    b.assign(G, {});
+    if (L.local) {
+      // (served below, without the exchange)
+    } else if (fits) {
+      for (uint32_t r = 0; r < G; r++) b[r].push_back(ShardBatch{rk[r].req, rk[r].dst, rk[r].out, n[r], round_up(maxc)});
+    } else {
+      // one source rank at a time sends pieces of at most min(cap, max_n) records, the others send empty batches:
+      // every shard still sees rank-major order, and a piece this small cannot overflow a slab
+      L.fallback_rounds++;
+      for (uint32_t src = 0; src < G; src++)
+        for (uint64_t from = 0; from < n[src]; from += piece) {
+          const uint64_t len = n[src] - from < piece ? n[src] - from : piece;
+          for (uint32_t r = 0; r < G; r++) {
+            const Rank& k = rk[r];
+            b[r].push_back(r == src ? ShardBatch{k.req + from * msg, k.dst ? k.dst + from : nullptr, k.out + from * msg, len, round_up(len)}
+                                    : ShardBatch{k.req, k.dst, k.out, 0, round_up(len)});
+          }
+        }
+    }
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventRecord(L.t_beg, L.mains[0]));
+    if (L.local) {
+      // log_server: a log record touches no keyed state, so its owner is the rank that received it (route_owner_of);
+      // serving each rank's batch on its own engine gives every shard the order the exchange would, without making
+      // each owner scan G - 1 slabs of padding
+      for (uint32_t r = 0; r < G; r++)
+        if (n[r]) {
+          CU(cudaSetDevice(cl->dev[r]));
+          if ((rc = run_device(cl->eng[r], rk[r].req, n[r], rk[r].out, L.mains[r]))) return rc;
+        }
+    } else {
+      const uint32_t k = (uint32_t)b[0].size();
+      if (k && (rc = shard_run(cl->sh.data(), G, k, b, L.mains.data()))) return rc;
+      for (uint32_t r = 0; r < G; r++) {          // the exchange flags of this round (dint_shard_flags, without its synchronise)
+        CU(cudaSetDevice(cl->dev[r]));
+        CU(cudaMemcpyAsync(rk[r].pub + 9, cl->sh[r]->flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, L.mains[r]));
+        CU(cudaMemsetAsync(cl->sh[r]->flags, 0, 2 * sizeof(uint32_t), L.mains[r]));
+      }
+    }
+    for (uint32_t r = 0; r < G; r++) { rk[r].last_n = n[r]; L.requests += n[r]; }
+    L.rounds++;
+    if ((rc = emit(0))) return rc;
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventRecord(L.t_end, L.mains[0]));
+    if ((rc = round_wait(L, rk))) return rc;
+    CU(cudaSetDevice(cl->dev[0]));
+    CU(cudaEventSynchronize(L.t_end));
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, L.t_beg, L.t_end));
+    const auto now = std::chrono::steady_clock::now();
+    L.wall_s += std::chrono::duration<double>(now - t_prev).count();
+    L.dev_s += ms * 1e-3;
+    L.timed++;
+    t_prev = now;
+  }
+  if ((rc = round_errors(cl, &err_after))) return rc;
+  return err_after != err_before ? set_err(DINT_EPROTO, "an engine answered a request with an error reply") : DINT_OK;
+}
+
+extern "C" {
+// ---- TATP / SmallBank closed-loop clients on the GPU against a shard cluster (txn_clients.cuh) ---------------
+// Every shard sees its records in the order one host TxnWorkload would send them.  A round's emission is three kernels
+// per rank: step / scan / compact leave the round in req[] / dst[] and its size and per-shard counts in pub.
+struct TxnRank : RoundRank {
+  txn::DevClients d{};
+  uint32_t tiles = 0;
+};
+struct dint_txn_clients : RoundLoop {
+  uint32_t n = 0;
+  std::vector<TxnRank> rk;
 };
 
 void dint_txn_clients_destroy(dint_txn_clients* t) {
@@ -1924,8 +2071,7 @@ int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0,
   *out = nullptr;
   if ((cl->kind != DINT_TATP && cl->kind != DINT_SMALLBANK) || n_clients == 0 || subscribers < 3)
     return set_err(DINT_EINVAL, "a tatp or smallbank cluster, n_clients > 0, subscribers >= 3");
-  // fallback pieces start at multiples of 16 records, so that every device batch stays 16-byte aligned
-  if (((cl->cap < cl->max_n ? cl->cap : cl->max_n) & ~15ull) == 0) return set_err(DINT_EINVAL, "the cluster's max_batch must be >= 16");
+  if (fallback_piece(cl) == 0) return set_err(DINT_EINVAL, "the cluster's max_batch must be >= 16");
   const uint32_t G = cl->G, msg = kMsgSize[cl->kind];
   dint_txn_clients* t = new dint_txn_clients();
   t->cl = cl; t->msg = msg; t->n = n_clients;
@@ -1961,6 +2107,7 @@ int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0,
     if (ce == cudaSuccess) ce = cudaHostAlloc(&k.pub, 16 * sizeof(uint32_t), cudaHostAllocMapped | cudaHostAllocPortable);
     if (ce != cudaSuccess) return fail(DINT_ENOMEM, "txn client state", ce);
     memset(k.pub, 0, 16 * sizeof(uint32_t));
+    k.req = k.d.req; k.dst = k.d.dst;
     if (ce == cudaSuccess) ce = cudaHostGetDevicePointer((void**)&k.d.pub, k.pub, 0);
     if (ce == cudaSuccess) ce = cudaMemset(k.d.cl, 0, n * csz + 16);
     if (ce == cudaSuccess) ce = cudaMemset(k.d.owner_cnt, 0, 8 * sizeof(uint32_t));
@@ -1998,95 +2145,10 @@ static int txn_emit(dint_txn_clients* t, int first) {
   t->started = true;
   return DINT_OK;
 }
-// wait for every rank's pending emission; the exchange flags of the round before it must read zero
-static int txn_wait(dint_txn_clients* t) {
-  for (uint32_t r = 0; r < t->cl->G; r++) {
-    CU(cudaSetDevice(t->cl->dev[r]));
-    CU(cudaEventSynchronize(t->rk[r].ev));
-  }
-  for (uint32_t r = 0; r < t->cl->G; r++)
-    if (t->rk[r].pub[9] || t->rk[r].pub[10]) return set_err(DINT_EIO, "internal: an exchange slab overflowed or a wait timed out");
-  return DINT_OK;
-}
-static int txn_errors(dint_txn_clients* t, unsigned long long* sum) {
-  *sum = 0;
-  for (auto* e : t->cl->eng) {
-    CU(cudaSetDevice(e->device));
-    int rc = pull_counters(e);
-    if (rc) return rc;
-    *sum += e->stats.errors;
-  }
-  return DINT_OK;
-}
 
 int dint_txn_clients_run(dint_txn_clients* t, uint32_t rounds) {
   if (!t) return set_err(DINT_EINVAL, "null argument");
-  dint_cluster* cl = t->cl;
-  const uint32_t G = cl->G, msg = t->msg;
-  unsigned long long err_before = 0, err_after = 0;
-  int rc = txn_errors(t, &err_before);
-  if (rc) return rc;
-  if (!t->started && (rc = txn_emit(t, 1))) return rc;
-  if ((rc = txn_wait(t))) return rc;
-  const uint32_t piece = (uint32_t)((cl->cap < cl->max_n ? cl->cap : cl->max_n) & ~15ull);
-  auto round_up = [](uint64_t x) { return (uint32_t)(x ? (x + kTile - 1) / kTile * kTile : kTile); };
-  std::vector<uint64_t> n(G);
-  std::vector<std::vector<ShardBatch>> b;
-  auto t_prev = std::chrono::steady_clock::now();
-  for (uint32_t i = 0; i < rounds; i++) {
-    // the slab capacity of the round: the largest (source, owner) count, so no slab can overflow
-    uint64_t maxc = 0;
-    bool fits = true;
-    for (uint32_t r = 0; r < G; r++) {
-      n[r] = t->rk[r].pub[0];
-      if (n[r] > cl->max_n) fits = false;
-      for (uint32_t o = 0; o < G; o++) maxc = t->rk[r].pub[1 + o] > maxc ? t->rk[r].pub[1 + o] : maxc;
-    }
-    if (maxc > cl->cap) fits = false;
-    b.assign(G, {});
-    if (fits) {
-      for (uint32_t r = 0; r < G; r++) b[r].push_back(ShardBatch{t->rk[r].d.req, t->rk[r].d.dst, t->rk[r].out, n[r], round_up(maxc)});
-    } else {
-      // one source rank at a time sends pieces of at most min(cap, max_n) records, the others send empty batches:
-      // every shard still sees rank-major order, and a piece this small cannot overflow a slab
-      t->fallback_rounds++;
-      for (uint32_t src = 0; src < G; src++)
-        for (uint64_t from = 0; from < n[src]; from += piece) {
-          const uint64_t len = n[src] - from < piece ? n[src] - from : piece;
-          for (uint32_t r = 0; r < G; r++) {
-            const TxnRank& k = t->rk[r];
-            b[r].push_back(r == src ? ShardBatch{k.d.req + from * msg, k.d.dst + from, k.out + from * msg, len, round_up(len)}
-                                    : ShardBatch{k.d.req, k.d.dst, k.out, 0, round_up(len)});
-          }
-        }
-    }
-    CU(cudaSetDevice(cl->dev[0]));
-    CU(cudaEventRecord(t->t_beg, t->mains[0]));
-    const uint32_t k = (uint32_t)b[0].size();
-    if (k && (rc = shard_run(cl->sh.data(), G, k, b, t->mains.data()))) return rc;
-    for (uint32_t r = 0; r < G; r++) {          // the exchange flags of this round (dint_shard_flags, without its synchronise)
-      CU(cudaSetDevice(cl->dev[r]));
-      CU(cudaMemcpyAsync(t->rk[r].pub + 9, cl->sh[r]->flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, t->mains[r]));
-      CU(cudaMemsetAsync(cl->sh[r]->flags, 0, 2 * sizeof(uint32_t), t->mains[r]));
-    }
-    for (uint32_t r = 0; r < G; r++) { t->rk[r].last_n = n[r]; t->requests += n[r]; }
-    t->rounds++;
-    if ((rc = txn_emit(t, 0))) return rc;
-    CU(cudaSetDevice(cl->dev[0]));
-    CU(cudaEventRecord(t->t_end, t->mains[0]));
-    if ((rc = txn_wait(t))) return rc;
-    CU(cudaSetDevice(cl->dev[0]));
-    CU(cudaEventSynchronize(t->t_end));
-    float ms = 0;
-    CU(cudaEventElapsedTime(&ms, t->t_beg, t->t_end));
-    const auto now = std::chrono::steady_clock::now();
-    t->wall_s += std::chrono::duration<double>(now - t_prev).count();
-    t->dev_s += ms * 1e-3;
-    t->timed++;
-    t_prev = now;
-  }
-  if ((rc = txn_errors(t, &err_after))) return rc;
-  return err_after != err_before ? set_err(DINT_EPROTO, "an engine answered a request with an error reply") : DINT_OK;
+  return serve_rounds(*t, t->rk, rounds, [t](int first) { return txn_emit(t, first); });
 }
 
 // out: dint_txn_stats' 18 words (requests and rounds served, transactions started, committed, started-by-type[7],
@@ -2117,7 +2179,7 @@ int dint_txn_clients_peek(dint_txn_clients* t, void* next_req, uint8_t* next_dst
   if (!t) return set_err(DINT_EINVAL, "null argument");
   int rc;
   if (!t->started && (rc = txn_emit(t, 1))) return rc;
-  if ((rc = txn_wait(t))) return rc;
+  if ((rc = round_wait(*t, t->rk))) return rc;
   uint64_t a = 0, z = 0;
   for (uint32_t r = 0; r < t->cl->G; r++) {
     const TxnRank& k = t->rk[r];
@@ -2136,6 +2198,152 @@ int dint_txn_clients_peek(dint_txn_clients* t, void* next_req, uint8_t* next_dst
 
 // out: rounds timed, their wall time on the host (s), and the CUDA-event time of their device work on rank 0 (s)
 int dint_txn_clients_times(dint_txn_clients* t, double out[3]) {
+  if (!t || !out) return set_err(DINT_EINVAL, "null argument");
+  out[0] = (double)t->timed; out[1] = t->wall_s; out[2] = t->dev_s;
+  return DINT_OK;
+}
+
+// ---- lock_2pl / lock_fasst / store / log_server closed-loop clients on the GPU against a shard cluster -------------
+// Rank r's block of clients (clients.cuh, ClientCtx::id0 = its first global id) emits one record per client into its
+// request buffer; k_clients_owner_count publishes the round's per-owner counts; the round loop above serves it; the
+// replies land in the block's reply buffer, in request order, where the next step absorbs them.  A cluster of these kinds
+// answers like ONE sequential server fed the rank-major concatenation, so the clients take, round for round, the
+// decisions of dint_clients with the same clients on one engine.
+struct ClusterClientRank : RoundRank {
+  ClientBlock b;                 // req = b.req, out = b.resp
+  uint32_t* acc = nullptr;       // k_clients_owner_count's per-shard sums [8] and CTA ticket [1]
+  uint32_t* pub_dev = nullptr;   // device view of pub
+};
+struct dint_cluster_clients : RoundLoop {
+  int kind = 0;
+  uint64_t seed = 0;
+  std::vector<ClusterClientRank> rk;
+};
+
+void dint_cluster_clients_destroy(dint_cluster_clients* t) {
+  if (!t) return;
+  for (size_t r = 0; r < t->rk.size(); r++) {
+    ClusterClientRank& k = t->rk[r];
+    cudaSetDevice(t->cl->dev[r]);
+    cudaDeviceSynchronize();
+    client_block_free(k.b);
+    cudaFree(k.acc);
+    if (k.pub) cudaFreeHost(k.pub);
+    if (k.ev) cudaEventDestroy(k.ev);
+  }
+  if (!t->rk.empty()) cudaSetDevice(t->cl->dev[0]);
+  if (t->t_beg) cudaEventDestroy(t->t_beg);
+  if (t->t_end) cudaEventDestroy(t->t_end);
+  delete t;
+}
+
+int dint_cluster_clients_create(dint_cluster* cl, const dint_clients_cfg* cfg, dint_cluster_clients** out) {
+  if (!cl || !cfg || !out) return set_err(DINT_EINVAL, "null argument");
+  *out = nullptr;
+  const uint32_t G = cl->G, n_clients = cfg->n_clients;
+  auto lo_of = [&](uint32_t r) { return (uint32_t)((uint64_t)n_clients * r / G); };
+  for (uint32_t r = 0; r < G; r++)                     // otherwise every round would be served in pieces
+    if (lo_of(r + 1) - lo_of(r) > cl->max_n) return set_err(DINT_EINVAL, "a rank's block of clients exceeds the cluster's max_batch");
+  if (fallback_piece(cl) == 0) return set_err(DINT_EINVAL, "the cluster's max_batch must be >= 16");
+  dint_cluster_clients* t = new dint_cluster_clients();
+  t->cl = cl; t->kind = cl->kind; t->msg = kMsgSize[cl->kind]; t->seed = cfg->seed; t->local = cl->kind == DINT_LOG;
+  t->rk.resize(G);
+  auto fail = [&](int code) { std::string keep = g_last_error; dint_cluster_clients_destroy(t); g_last_error = keep; return code; };
+  for (uint32_t r = 0; r < G; r++) {
+    ClusterClientRank& k = t->rk[r];
+    const uint32_t lo = lo_of(r), n = lo_of(r + 1) - lo;
+    t->mains.push_back(cl->shared_device ? cl->eng[0]->stream : cl->eng[r]->stream);
+    if (int rc = client_block_make(cl->kind, cfg, cl->dev[r], lo, n, &k.b)) return fail(rc);
+    k.req = k.b.req; k.out = k.b.resp;
+    cudaError_t ce = cudaSetDevice(cl->dev[r]);
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.acc, 16 * sizeof(uint32_t));
+    if (ce == cudaSuccess) ce = cudaMemset(k.acc, 0, 16 * sizeof(uint32_t));
+    if (ce == cudaSuccess) ce = cudaHostAlloc(&k.pub, 16 * sizeof(uint32_t), cudaHostAllocMapped | cudaHostAllocPortable);
+    if (ce != cudaSuccess) return fail(set_err(DINT_ENOMEM, "cluster client state", ce));
+    memset(k.pub, 0, 16 * sizeof(uint32_t));
+    k.pub[0] = n;                                      // (log_server rounds are not counted: their size is the block's)
+    if (ce == cudaSuccess) ce = cudaHostGetDevicePointer((void**)&k.pub_dev, k.pub, 0);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&k.ev, cudaEventDisableTiming);
+    if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
+    if (ce != cudaSuccess) return fail(set_err(DINT_EIO, "cluster client setup", ce));
+  }
+  cudaError_t ce = cudaSetDevice(cl->dev[0]);
+  if (ce == cudaSuccess) ce = cudaEventCreate(&t->t_beg);
+  if (ce == cudaSuccess) ce = cudaEventCreate(&t->t_end);
+  if (ce != cudaSuccess) return fail(set_err(DINT_EIO, "cluster client events", ce));
+  *out = t;
+  return DINT_OK;
+}
+
+// enqueue one emission on every rank: the clients' kernel, then (except log_server) the per-owner count
+static int cluster_clients_emit(dint_cluster_clients* t, int first) {
+  dint_cluster* cl = t->cl;
+  for (uint32_t r = 0; r < cl->G; r++) {
+    ClusterClientRank& k = t->rk[r];
+    dint_engine* e = cl->eng[r];
+    CU(cudaSetDevice(cl->dev[r]));
+    const cudaStream_t s = t->mains[r];
+    const uint32_t n = k.b.cc.n_clients, blocks = (n + kThreads - 1) / kThreads;
+    if (n) {
+      clients_launch(t->kind, t->seed, k.b, first != 0, s);
+      e->stats.kernel_launches++;
+      if (!t->local) {
+        switch (t->kind) {
+          case DINT_FASST: k_clients_owner_count<K_FASST><<<blocks, kThreads, 0, s>>>(e->ctx, k.b.req, n, k.acc, k.pub_dev); break;
+          case DINT_LOCK2PL: k_clients_owner_count<K_LOCK2PL><<<blocks, kThreads, 0, s>>>(e->ctx, k.b.req, n, k.acc, k.pub_dev); break;
+          default: k_clients_owner_count<K_STORE><<<blocks, kThreads, 0, s>>>(e->ctx, k.b.req, n, k.acc, k.pub_dev); break;
+        }
+        e->stats.kernel_launches++;
+      }
+    }
+    CU(cudaEventRecord(k.ev, s));
+  }
+  CU(cudaGetLastError());
+  t->started = true;
+  return DINT_OK;
+}
+
+int dint_cluster_clients_run(dint_cluster_clients* t, uint32_t rounds) {
+  if (!t) return set_err(DINT_EINVAL, "null argument");
+  return serve_rounds(*t, t->rk, rounds, [t](int first) { return cluster_clients_emit(t, first); });
+}
+
+// out: dint_clients_stats_all's 6 words (rounds counted once, not once per rank), then rounds served in pieces
+int dint_cluster_clients_stats(dint_cluster_clients* t, uint64_t out[7]) {
+  if (!t || !out) return set_err(DINT_EINVAL, "null argument");
+  unsigned long long s[6] = {0};
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    unsigned long long h[6];
+    CU(cudaSetDevice(t->cl->dev[r]));
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(h, t->rk[r].b.cc.stats, sizeof h, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < 6; i++) s[i] += h[i];
+  }
+  out[0] = s[0]; out[1] = s[1]; out[2] = s[2]; out[3] = s[3]; out[4] = s[5]; out[5] = t->rounds; out[6] = t->fallback_rounds;
+  return DINT_OK;
+}
+
+// test hook, global client order: the requests the clients send next and the replies they absorbed last (host buffers
+// of n_clients * dint_msg_size(kind) bytes)
+int dint_cluster_clients_peek(dint_cluster_clients* t, void* next_req, void* last_resp) {
+  if (!t) return set_err(DINT_EINVAL, "null argument");
+  int rc;
+  if (!t->started && (rc = cluster_clients_emit(t, 1))) return rc;
+  if ((rc = round_wait(*t, t->rk))) return rc;
+  uint64_t a = 0;
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    const ClusterClientRank& k = t->rk[r];
+    const size_t bytes = (size_t)k.b.cc.n_clients * t->msg;
+    CU(cudaSetDevice(t->cl->dev[r]));
+    if (next_req && bytes) CU(cudaMemcpy((uint8_t*)next_req + a, k.b.req, bytes, cudaMemcpyDeviceToHost));
+    if (last_resp && bytes) CU(cudaMemcpy((uint8_t*)last_resp + a, k.b.resp, bytes, cudaMemcpyDeviceToHost));
+    a += bytes;
+  }
+  return DINT_OK;
+}
+
+// out: rounds timed, their wall time on the host (s), and the CUDA-event time of their device work on rank 0 (s)
+int dint_cluster_clients_times(dint_cluster_clients* t, double out[3]) {
   if (!t || !out) return set_err(DINT_EINVAL, "null argument");
   out[0] = (double)t->timed; out[1] = t->wall_s; out[2] = t->dev_s;
   return DINT_OK;

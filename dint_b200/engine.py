@@ -56,7 +56,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -115,6 +115,12 @@ def lib():
     L.dint_txn_clients_peek.restype = i32; L.dint_txn_clients_peek.argtypes = [vp, vp, vp, C.POINTER(u64), vp, C.POINTER(u64)]
     L.dint_txn_clients_times.restype = i32; L.dint_txn_clients_times.argtypes = [vp, C.POINTER(C.c_double)]
     L.dint_txn_clients_destroy.restype = None; L.dint_txn_clients_destroy.argtypes = [vp]
+    L.dint_cluster_clients_create.restype = i32; L.dint_cluster_clients_create.argtypes = [vp, C.POINTER(DintClientsCfg), C.POINTER(vp)]
+    L.dint_cluster_clients_run.restype = i32; L.dint_cluster_clients_run.argtypes = [vp, u32]
+    L.dint_cluster_clients_stats.restype = i32; L.dint_cluster_clients_stats.argtypes = [vp, C.POINTER(u64)]
+    L.dint_cluster_clients_peek.restype = i32; L.dint_cluster_clients_peek.argtypes = [vp, vp, vp]
+    L.dint_cluster_clients_times.restype = i32; L.dint_cluster_clients_times.argtypes = [vp, C.POINTER(C.c_double)]
+    L.dint_cluster_clients_destroy.restype = None; L.dint_cluster_clients_destroy.argtypes = [vp]
     L.dint_snapshot_create.restype = i32; L.dint_snapshot_create.argtypes = [vp, C.POINTER(vp)]
     L.dint_snapshot_restore.restype = i32; L.dint_snapshot_restore.argtypes = [vp, vp]
     L.dint_snapshot_destroy.restype = None; L.dint_snapshot_destroy.argtypes = [vp]
@@ -608,6 +614,77 @@ class GpuTxnClients:
     def close(self):
         if getattr(self, "h", None):
             lib().dint_txn_clients_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class GpuClusterClients:
+    """lock_2pl, lock_fasst, store or log_server closed-loop clients resident on the GPUs of `cluster` (a GpuCluster of
+    that kind; dint_cluster_clients_*): GpuClients' state machines, split over the ranks in contiguous blocks, every
+    round served by one exchange step.  The keyword arguments are those of GpuClients and workloads.Workload, and the
+    clients send and absorb, round for round, what GpuClients with the same clients on one engine would.  Keep the
+    cluster open while these clients exist."""
+
+    def __init__(self, cluster, n_clients, seed=20230, n_keys=24_000_000, zipf_theta=0.0, read_pct=80, set_pct=0,
+                 store_subscribers=2_000_000, store_hot=False):
+        self.cluster, self.n, self.kind, self.msg = cluster, n_clients, cluster.kind, cluster.msg
+        cfg = DintClientsCfg(n_clients=n_clients, n_keys=n_keys, seed=seed, zipf_theta=zipf_theta, read_pct=read_pct,
+                             set_pct=set_pct, store_subscribers=store_subscribers, store_hot=1 if store_hot else 0)
+        h = C.c_void_p()
+        rc = lib().dint_cluster_clients_create(cluster.h, C.byref(cfg), C.byref(h))
+        if rc != 0:
+            raise DintError(rc, "dint_cluster_clients_create")
+        self.h = h
+
+    def run(self, rounds, check=True):
+        """Serve `rounds` closed-loop rounds; returns when they are served."""
+        rc = lib().dint_cluster_clients_run(self.h, rounds)
+        if rc != 0 and (check or rc != DINT_EPROTO):
+            raise DintError(rc, "dint_cluster_clients_run")
+        return rc
+
+    def stats(self):
+        """GpuClients.stats()'s dict (rounds counted once, not once per rank) plus fallback_rounds, the rounds served
+        in pieces because some (rank, shard) count exceeded the cluster's slab capacity."""
+        out = (C.c_uint64 * 7)()
+        rc = lib().dint_cluster_clients_stats(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_cluster_clients_stats")
+        keys = ["requests", "committed", "validation_aborts", "lock_rejects", "not_exist", "rounds", "fallback_rounds"]
+        return dict(zip(keys, [int(x) for x in out]))
+
+    def peek(self):
+        """(the requests the clients send next, the replies they absorbed last) in global client order: uint8 arrays of
+        n_clients * msg bytes"""
+        rq = np.empty(self.n * self.msg, dtype=np.uint8)
+        rs = np.empty(self.n * self.msg, dtype=np.uint8)
+        rc = lib().dint_cluster_clients_peek(self.h, rq.ctypes.data, rs.ctypes.data)
+        if rc != 0:
+            raise DintError(rc, "dint_cluster_clients_peek")
+        return rq, rs
+
+    def times(self):
+        """Rounds timed by run(), their host wall time and the CUDA-event time of their device work (rank 0), in s."""
+        out = (C.c_double * 3)()
+        rc = lib().dint_cluster_clients_times(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_cluster_clients_times")
+        return {"rounds": int(out[0]), "wall_s": out[1], "device_s": out[2]}
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().dint_cluster_clients_destroy(self.h)
             self.h = None
 
     def __enter__(self):

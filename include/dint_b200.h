@@ -339,6 +339,37 @@ int dint_txn_clients_peek(dint_txn_clients *t, void *next_req, uint8_t *next_dst
 int dint_txn_clients_times(dint_txn_clients *t, double out[3]);
 void dint_txn_clients_destroy(dint_txn_clients *t);
 
+/*
+ * lock_2pl, lock_fasst, store and log_server closed-loop clients ON the GPU, against a shard cluster: the clients of
+ * dint_clients_create_cfg (same family fields, same draws and decisions), with the kind and shard count taken from the
+ * cluster.  Clients [0, n_clients) are split over the ranks in contiguous blocks, rank r's block on rank r's device (a
+ * rank may hold none).  A cluster of these kinds answers like ONE sequential server fed the rank-major concatenation, so
+ * the clients send and absorb, round for round, exactly what dint_clients with the same clients on one engine would.
+ * The cluster must outlive the clients.
+ *   dint_cluster_clients_create: DINT_EINVAL for a tatp / smallbank cluster (their clients: dint_txn_clients_*), for
+ *     every argument dint_clients_create_cfg refuses, and when a rank's block (n_clients / shards, rounded up) exceeds
+ *     the cluster's max_batch -- every round would then be served in pieces.
+ *   dint_cluster_clients_run (blocking): `rounds` rounds.  Each rank's clients emit one record each and a kernel counts
+ *     them per owner shard; one host synchronise per round reads the counts, which size the exchange slabs exactly, and
+ *     one exchange step serves the round.  A round whose largest (rank, shard) count exceeds the cluster's slab capacity
+ *     is served one source rank at a time, in pieces (counted in stats[6]).  log_server rounds skip the exchange (a log
+ *     record is owned by the rank that received it): each rank's engine serves its own batch.  Returns 0, DINT_EPROTO
+ *     (an engine answered with an error reply), or an error.
+ *   dint_cluster_clients_stats (synchronises): dint_clients_stats_all's 6 words (rounds counted once, not per rank),
+ *     then rounds served in pieces.
+ *   dint_cluster_clients_peek (test hook, synchronises): in global client order, the next round's requests / the last
+ *     round's replies, n_clients * dint_msg_size(kind) bytes each.
+ *   dint_cluster_clients_times: as dint_txn_clients_times.
+ * The first round is emitted by the first run or peek call.
+ */
+typedef struct dint_cluster_clients dint_cluster_clients;
+int dint_cluster_clients_create(dint_cluster *c, const dint_clients_cfg *cfg, dint_cluster_clients **out);
+int dint_cluster_clients_run(dint_cluster_clients *t, uint32_t rounds);
+int dint_cluster_clients_stats(dint_cluster_clients *t, uint64_t out[7]);
+int dint_cluster_clients_peek(dint_cluster_clients *t, void *next_req, void *last_resp);
+int dint_cluster_clients_times(dint_cluster_clients *t, double out[3]);
+void dint_cluster_clients_destroy(dint_cluster_clients *t);
+
 int dint_get_stats(dint_engine *e, dint_stats *s);
 void dint_reset_stats(dint_engine *e);
 /* per-kernel CUDA-event timing: 0 = off, 1 = every kernel, otherwise a bit mask over

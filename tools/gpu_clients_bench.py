@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Live lock_2pl / store / log_server / lock_fasst closed loops on the GPU (GpuClients), one engine per workload.
+"""Live lock_2pl / store / log_server / lock_fasst closed loops on the GPU (GpuClients), one engine per workload, or
+against a shard cluster (GpuClusterClients, --shards).
 
 2^20 clients per workload at the reference's sizes:
   lock2pl_ref       lock_2pl, 24,000,000 ids uniform on 36,000,000 lock slots
@@ -21,6 +22,7 @@ import json
 import math
 import os
 import sys
+import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -90,6 +92,56 @@ def check(name, clients, rounds):
     return {"check_rounds": rounds, "check_identical": got == want, "check_stats": got}
 
 
+def measure_cluster(name, clients, G, devices, warmup, min_seconds):
+    import torch
+    from dint_b200 import GpuCluster, GpuClusterClients, wire
+    kind_name, eng_opt, fam = WORKLOADS[name]
+    kind = getattr(wire, kind_name)
+    res = {"workload": name, "kind": wire.KIND_NAMES[kind], "clients": clients * G, "clients_per_rank": clients,
+           "shards": G, "devices": devices, "family": fam}
+    with GpuCluster(kind, G, devices=devices, max_batch=clients, **eng_opt) as cl, \
+            GpuClusterClients(cl, clients * G, seed=SEED, **fam) as cc:
+        cc.run(warmup)
+        s0, m0 = cc.stats(), cc.times()
+        rounds, t0 = 0, time.perf_counter()
+        while True:
+            cc.run(10)
+            rounds += 10
+            wall = time.perf_counter() - t0
+            if wall >= min_seconds:
+                break
+        torch.cuda.synchronize()
+        s1, m1 = cc.stats(), cc.times()
+        res["card_after_timed"] = card()              # the SM clock while the card is still warm
+    dwall, ddev = m1["wall_s"] - m0["wall_s"], m1["device_s"] - m0["device_s"]
+    d = {k: s1[k] - s0[k] for k in s1}
+    res.update(rounds_timed=rounds, timed_s=round(wall, 4), txn_per_s=d["committed"] / wall, requests_per_s=d["requests"] / wall,
+               us_per_round=1e6 * wall / rounds, round_device_us=1e6 * ddev / rounds,
+               exposed_host_us_per_round=1e6 * (dwall - ddev) / rounds, fallback_rounds=d["fallback_rounds"],
+               committed=d["committed"], validation_aborts=d["validation_aborts"], lock_rejects=d["lock_rejects"],
+               not_exist=d["not_exist"])
+    print(f"[{name}] {G} shards: {rounds} rounds in {wall:.3f} s", flush=True)
+    return res
+
+
+def check_cluster(name, clients, G, devices, rounds):
+    """the first `rounds` rounds: cluster clients vs GpuClients with the same clients on one engine"""
+    import numpy as np
+    from dint_b200 import Engine, GpuCluster, GpuClients, GpuClusterClients, wire
+    kind_name, eng_opt, fam = WORKLOADS[name]
+    kind = getattr(wire, kind_name)
+    with GpuCluster(kind, G, devices=devices, max_batch=clients, **eng_opt) as cl, \
+            GpuClusterClients(cl, clients * G, seed=SEED, **fam) as cc:
+        cc.run(rounds)
+        got, got_io = cc.stats(), cc.peek()
+    with Engine(kind, **eng_opt) as eng, GpuClients(eng, clients * G, seed=SEED, **fam) as gc:
+        gc.run(rounds)
+        want, want_io = gc.stats(), gc.peek()
+    same = {k: v for k, v in got.items() if k != "fallback_rounds"} == want and \
+        all(np.array_equal(a, b) for a, b in zip(got_io, want_io))
+    return {"check_rounds": rounds, "check_identical": same, "check_stats": got}
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
@@ -97,19 +149,35 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--min-seconds", type=float, default=1.0)
     ap.add_argument("--check", type=int, default=0, metavar="R")
+    ap.add_argument("--shards", type=int, default=0, metavar="G")
+    ap.add_argument("--devices", default=None, metavar="d0,d1,...")
     a = ap.parse_args()
     names = a.workloads.split(",")
     for n in names:
         if n not in WORKLOADS:
             ap.error(f"unknown workload {n!r}; known: {', '.join(WORKLOADS)}")
+    devices = None
+    if a.shards:
+        devices = [int(d) for d in a.devices.split(",")] if a.devices else [0] * a.shards
+        if len(devices) != a.shards:
+            ap.error("--devices must name one device per shard")
+    elif a.devices:
+        ap.error("--devices needs --shards")
     print(json.dumps({"card": card()}), flush=True)
     ok = True
     for n in names:
-        r = measure(n, a.clients, a.warmup, a.min_seconds)
+        if a.shards:
+            r = measure_cluster(n, a.clients, a.shards, devices, a.warmup, a.min_seconds)
+            if a.check:
+                r.update(check_cluster(n, a.clients, a.shards, devices, a.check))
+        else:
+            r = measure(n, a.clients, a.warmup, a.min_seconds)
+            if a.check:
+                r.update(check(n, a.clients, a.check))
         if a.check:
-            r.update(check(n, a.clients, a.check))
             ok &= r["check_identical"]
         print(f"[{n}] {r['txn_per_s'] / 1e6:.2f} M txn/s, {r['requests_per_s'] / 1e6:.1f} M req/s, {r['us_per_round']:.0f} us/round"
+              + (f", {r['exposed_host_us_per_round']:.0f} us exposed host, {r['fallback_rounds']} fallback rounds" if a.shards else "")
               + (f" | check of {a.check} rounds identical: {r['check_identical']}" if a.check else ""), flush=True)
         print(json.dumps(r), flush=True)
     sys.exit(0 if ok else 1)
