@@ -642,6 +642,9 @@ static int create_impl(dint_engine* e) {
   }
   e->total_groups = groups;
   if (groups >= 0xffffffffULL) return set_err(DINT_EINVAL, "too many groups");
+  // holder keys: plain HBM, outside the persisting window below -- only lock requests touch them, and the window is
+  // for what every request touches
+  if ((cf.flags & DINT_CFG_LOCK_HOLDER_KEYS) && (rc = dalloc(e, &c.holder, groups))) return rc;
   {
     uint32_t fl = 25;                                  // 2^25 nibbles = 16 MB per set: L2-resident
     while (fl > 10 && (1ULL << (fl - 1)) >= groups * 2 + 2048) fl--;   // tiny group spaces need less
@@ -728,6 +731,7 @@ int dint_create(int kind, const dint_cfg* cfg, int device, dint_engine** out) {
   dint_cfg& cf = e->cfg;
   if (cf.n_shards == 0) cf.n_shards = 1;
   if (cf.shard_id >= cf.n_shards || cf.lock_slots == 0) { delete e; return set_err(DINT_EINVAL, "bad shard/lock_slots"); }
+  if ((cf.flags & DINT_CFG_LOCK_HOLDER_KEYS) && kind != DINT_TATP) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_LOCK_HOLDER_KEYS is a tatp option"); }
   if (cf.chunk == 0) cf.chunk = 1u << 20;
   e->chunk = (cf.chunk + kTile - 1) / kTile * kTile;
   {
@@ -971,6 +975,7 @@ static void snapshot_regions(dint_engine* e, std::vector<std::pair<void*, size_t
   if (e->kind == DINT_LOCK2PL || e->kind == DINT_SMALLBANK) r.push_back({c.cnt2, g * sizeof(uint2)});
   if (e->kind == DINT_FASST) { r.push_back({c.ver, g * sizeof(uint32_t)}); r.push_back({c.lockbits, ((g + 31) / 32) * 4}); }
   if (e->kind == DINT_TATP) r.push_back({c.lockbits, ((g + 31) / 32) * 4});
+  if (c.holder) r.push_back({c.holder, g * sizeof(uint64_t)});
   for (uint32_t t = 0; t < c.n_tables; t++) {
     r.push_back({c.tbl[t].entries, (size_t)(c.tbl[t].cap_mask + 1) << c.tbl[t].ent_shift});
     r.push_back({c.tbl[t].live, 16});
@@ -1046,6 +1051,16 @@ int dint_lock_state(dint_engine* e, int table, uint32_t slot, uint32_t out[2]) {
     out[0] = (w >> (g & 31)) & 1u;
     if (e->kind == DINT_FASST) CU(cudaMemcpy(&out[1], c.ver + g, 4, cudaMemcpyDeviceToHost));
   }
+  return DINT_OK;
+}
+
+int dint_lock_holder(dint_engine* e, int table, uint32_t slot, uint64_t* key) {
+  if (!e || !key || !e->ctx.holder) return DINT_EINVAL;
+  const Ctx& c = e->ctx;
+  if (table < 0 || table >= (int)c.n_tables || slot % c.n_shards != c.shard_id || slot / c.n_shards >= c.tbl[table].n_groups) return DINT_EINVAL;
+  CU(cudaSetDevice(e->device));
+  CU(cudaDeviceSynchronize());
+  CU(cudaMemcpy(key, c.holder + c.tbl[table].grp_base + slot / c.n_shards, sizeof *key, cudaMemcpyDeviceToHost));
   return DINT_OK;
 }
 
@@ -1544,6 +1559,7 @@ int dint_cluster_create(int kind, const dint_cfg* cfg, int n_gpus, const int* de
   *out = nullptr;
   const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
   if (by_dst && n_gpus == 2) return set_err(DINT_EINVAL, "tatp / smallbank placement needs 1 or >= 3 shards (primary + 2 backups)");
+  if (cfg && (cfg->flags & DINT_CFG_LOCK_HOLDER_KEYS) && kind != DINT_TATP) return set_err(DINT_EINVAL, "DINT_CFG_LOCK_HOLDER_KEYS is a tatp option");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_err(DINT_ENODEV, "no CUDA device: dint_b200 has no CPU fallback"); }
   dint_cluster* cl = new dint_cluster();
@@ -2100,7 +2116,7 @@ int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0,
     if (ce == cudaSuccess) ce = cudaMalloc(&k.d.off, n * 4 + 16);
     if (ce == cudaSuccess) ce = cudaMalloc(&k.d.tile_sum, (size_t)k.tiles * 4 + 16);
     if (ce == cudaSuccess) ce = cudaMalloc(&k.d.owner_cnt, 8 * sizeof(uint32_t));
-    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.stats, 14 * sizeof(unsigned long long));
+    if (ce == cudaSuccess) ce = cudaMalloc(&k.d.stats, txn::kDevStats * sizeof(unsigned long long));
     if (ce == cudaSuccess) ce = cudaMalloc(&k.d.req, rec * msg + 16);
     if (ce == cudaSuccess) ce = cudaMalloc(&k.d.dst, rec + 16);
     if (ce == cudaSuccess) ce = cudaMalloc(&k.out, rec * msg + 16);
@@ -2111,7 +2127,7 @@ int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0,
     if (ce == cudaSuccess) ce = cudaHostGetDevicePointer((void**)&k.d.pub, k.pub, 0);
     if (ce == cudaSuccess) ce = cudaMemset(k.d.cl, 0, n * csz + 16);
     if (ce == cudaSuccess) ce = cudaMemset(k.d.owner_cnt, 0, 8 * sizeof(uint32_t));
-    if (ce == cudaSuccess) ce = cudaMemset(k.d.stats, 0, 14 * sizeof(unsigned long long));
+    if (ce == cudaSuccess) ce = cudaMemset(k.d.stats, 0, txn::kDevStats * sizeof(unsigned long long));
     if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&k.ev, cudaEventDisableTiming);
     if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
     if (ce != cudaSuccess) return fail(DINT_EIO, "txn client setup", ce);
@@ -2151,25 +2167,44 @@ int dint_txn_clients_run(dint_txn_clients* t, uint32_t rounds) {
   return serve_rounds(*t, t->rk, rounds, [t](int first) { return txn_emit(t, first); });
 }
 
+// the ranks' DevClients::stats words, summed (synchronises)
+static int txn_dev_stats(dint_txn_clients* t, unsigned long long by[txn::kDevStats]) {
+  if (!t->started) { int rc = txn_emit(t, 1); if (rc) return rc; }
+  for (uint32_t i = 0; i < txn::kDevStats; i++) by[i] = 0;
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    unsigned long long h[txn::kDevStats];
+    CU(cudaSetDevice(t->cl->dev[r]));
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(h, t->rk[r].d.stats, sizeof h, cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < txn::kDevStats; i++) by[i] += h[i];
+  }
+  return DINT_OK;
+}
+
 // out: dint_txn_stats' 18 words (requests and rounds served, transactions started, committed, started-by-type[7],
 // committed-by-type[7]), then rounds served through the fallback
 int dint_txn_clients_stats(dint_txn_clients* t, uint64_t out[19]) {
   if (!t || !out) return set_err(DINT_EINVAL, "null argument");
-  if (!t->started) { int rc = txn_emit(t, 1); if (rc) return rc; }
-  unsigned long long by[14] = {0};
-  for (uint32_t r = 0; r < t->cl->G; r++) {
-    unsigned long long h[14];
-    CU(cudaSetDevice(t->cl->dev[r]));
-    CU(cudaDeviceSynchronize());
-    CU(cudaMemcpy(h, t->rk[r].d.stats, sizeof h, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < 14; i++) by[i] += h[i];
-  }
+  unsigned long long by[txn::kDevStats];
+  int rc = txn_dev_stats(t, by);
+  if (rc) return rc;
   out[0] = t->requests; out[1] = 0; out[2] = 0; out[3] = t->rounds;
   for (int i = 0; i < 7; i++) {
     out[4 + i] = by[i]; out[11 + i] = by[7 + i];
     out[1] += by[i]; out[2] += by[7 + i];
   }
   out[18] = t->fallback_rounds;
+  return DINT_OK;
+}
+
+// out: kAcquireLock replies absorbed, of them kRejectLock (false sharing) and kRejectLockSameKey, as
+// tatp/caladan/client_lock.cc counts them
+int dint_txn_clients_lock_stats(dint_txn_clients* t, uint64_t out[3]) {
+  if (!t || !out) return set_err(DINT_EINVAL, "null argument");
+  unsigned long long by[txn::kDevStats];
+  int rc = txn_dev_stats(t, by);
+  if (rc) return rc;
+  for (int i = 0; i < 3; i++) out[i] = by[14 + i];
   return DINT_OK;
 }
 

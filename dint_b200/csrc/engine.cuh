@@ -128,6 +128,7 @@ struct Ctx {
   uint32_t* lockbits;      // fasst / tatp: 1 bit per group
   uint32_t* ver;           // fasst: u32 per slot
   uint2* cnt2;             // lock_2pl / smallbank: {num_ex, num_sh} per group
+  uint64_t* holder;        // tatp with DINT_CFG_LOCK_HOLDER_KEYS: key of the last granted acquire per group; else null
   // KV
   KvTable tbl[kMaxTables];
   uint32_t n_tables;

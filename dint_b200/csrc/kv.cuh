@@ -251,7 +251,14 @@ template <> DINT_D KeyInfo key_info<K_TATP>(const Ctx& c, const uint8_t* rec) {
   k.grp = kv_group(c, rec[W::TABLE], k.h);                          // lock_hash, tatp/udp/tatp.h:12-14
   return k;
 }
+// v: the key's home entry; for a kAcquireLock of an engine that keeps holder keys, v[0].x/.y = the group's holder word
 template <> struct Pre<K_TATP> { uint4 v[4]; };
+// The holder word (tatp/ebpf/lock_kern.c:12-16 `txn_lock.key`) belongs to resource L of its group: written by a granted
+// kAcquireLock, read by a refused one, both WL.  A solo acquire is the only WL request of its group in the chunk, so the
+// word fetched beside the flag lookup is the one its reply needs; two acquires of one group raise W2 and are replayed in
+// index order, each fetching the word after its predecessor was applied.
+DINT_D bool tatp_wants_holder(const Ctx& c, uint8_t type) { return type == 1 && c.holder != nullptr; }
+DINT_D uint2 tatp_load_holder(const Ctx& c, uint32_t g) { return __ldcg((const uint2*)(c.holder + g)); }
 DINT_D bool tatp_touches_row(uint8_t type) {   // request types that look a row up (not insert / lock / log)
   return type == 0 || type == 12 || type == 13 || type == 22 || type == 23;
 }
@@ -259,13 +266,18 @@ template <> DINT_D Pre<K_TATP> prefetch<K_TATP>(const Ctx& c, const uint8_t* rec
   using W = Wire<K_TATP>;
   Pre<K_TATP> p;
   if (tatp_touches_row(rec[W::TYPE])) kv_prefetch_home<40>(c, rec[W::TABLE], ki.h, p.v);
+  else if (tatp_wants_holder(c, rec[W::TYPE])) { const uint2 k = tatp_load_holder(c, ki.grp); p.v[0].x = k.x; p.v[0].y = k.y; }
   return p;
 }
 template <> DINT_D Pre<K_TATP> prefetch_coop<K_TATP>(const Ctx& c, const uint8_t* rec, const KeyInfo& ki, const TypeInfo&, bool active) {
   using W = Wire<K_TATP>;
   Pre<K_TATP> p;
   const bool need = active && tatp_touches_row(rec[W::TYPE]);
+  const bool lock = active && tatp_wants_holder(c, rec[W::TYPE]);
+  uint2 k = make_uint2(0, 0);
+  if (lock) k = tatp_load_holder(c, ki.grp);        // issued before the row fetch: the two latencies overlap
   kv_prefetch_home_coop<40>(need ? kv_home_ptr<40>(c, rec[W::TABLE], ki.h) : nullptr, need, p.v);
+  if (lock) { p.v[0].x = k.x; p.v[0].y = k.y; }
   return p;
 }
 template <>
@@ -298,7 +310,14 @@ DINT_D void apply_one<K_TATP>(const Ctx& c, uint8_t* rec, const KeyInfo& ki, con
   bool ok = true;
   switch (type) {
     case 0: rec[W::TYPE] = kv_get_into<40>(t, key, h, v, rec + W::VAL, rec + W::VER) ? 4 : 6; break;  // :116-121
-    case 1: rec[W::TYPE] = bm_fetch_set(c.lockbits, g) ? 8 : 7; break;                                // :123-132
+    case 1:                                                                                           // :123-132
+      if (!bm_fetch_set(c.lockbits, g)) {                    // granted; with holder keys, tatp/ebpf/lock_kern.c:290-293
+        if (c.holder) __stcg((uint2*)(c.holder + g), make_uint2((uint32_t)key, (uint32_t)(key >> 32)));
+        rec[W::TYPE] = 7;
+      } else {                                               // :294-298: kRejectLockSameKey when the holder's key is ours
+        rec[W::TYPE] = (c.holder && v[0].x == (uint32_t)key && v[0].y == (uint32_t)(key >> 32)) ? 28 : 8;
+      }
+      break;
     case 2: bm_clear_bit(c.lockbits, g); rec[W::TYPE] = 9; break;                                     // :134-138
     // a would-panic request (kvs_set / kvs_delete on a missing key) applies NOTHING: the reference dies before the unlock
     case 12: ok = kv_set_from<40>(t, key, h, v, rec + W::VAL); if (ok) bm_clear_bit(c.lockbits, g); rec[W::TYPE] = 15; break;  // :140-146

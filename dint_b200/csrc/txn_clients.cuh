@@ -14,8 +14,9 @@
 // Sharding generalised from 3 to G shards (SURVEY.md section 8(e)): primary p = key % G, backups (p+1) % G and
 // (p+2) % G, log records to those same three; G = 3 is exactly the reference.
 //
-// Statistics go to a Sink: begin(type) when a transaction starts, commit(type) when one commits.  One absorb finishes
-// at most one transaction and starts at most one, which the device sink relies on.
+// Statistics go to a Sink: begin(type) when a transaction starts, commit(type) when one commits, lock_reply(type) for
+// every absorbed reply to a TATP kAcquireLock.  One absorb finishes at most one transaction, starts at most one and
+// sees at most two lock replies, which the device sink relies on.
 //
 // Under nvcc the kernels of the on-GPU clients follow (one thread per client; see the comment above them).
 #pragma once
@@ -53,8 +54,9 @@ constexpr uint32_t kSeedBase = 0xdeadbeefu;   // client_udp_shard.cc:1121: seed 
 // ================================================ TATP ==============================================
 // wire: {ord@0, type@1, table@2, key@3, val@11[40], ver@51}  (tatp/udp/net.h:57-65)
 constexpr int TM = 55;
+// T_REJECT_LOCK_SAME_KEY: only servers that keep holder keys send it (tatp/ebpf/lock_kern.c:297-298, proto.h:52)
 enum { T_READ = 0, T_LOCK = 1, T_ABORT = 2, T_GRANT_READ = 4, T_NOT_EXIST = 6, T_GRANT_LOCK = 7, T_REJECT_LOCK = 8,
-       T_COMMIT_PRIM = 12, T_COMMIT_BCK = 13, T_COMMIT_LOG = 14, T_INSERT_PRIM = 18, T_INSERT_BCK = 19,
+       T_REJECT_LOCK_SAME_KEY = 28, T_COMMIT_PRIM = 12, T_COMMIT_BCK = 13, T_COMMIT_LOG = 14, T_INSERT_PRIM = 18, T_INSERT_BCK = 19,
        T_DELETE_PRIM = 22, T_DELETE_BCK = 23, T_DELETE_LOG = 24 };
 enum { TB_SUB = 0, TB_SEC = 1, TB_ACC = 2, TB_SF = 3, TB_CF = 4 };
 enum { X_GET_SUB = 0, X_GET_ACC, X_GET_DEST, X_UPD_SUB, X_UPD_LOC, X_INS_CF, X_DEL_CF };
@@ -281,6 +283,10 @@ TXN_HD void tatp_emit(const Cfg& w, TatpClient& c, Out& o) {
 TXN_HD void tatp_load(TMsg& m, const uint8_t* r, int i) { memcpy(m.b, r + (size_t)i * TM, TM); }
 TXN_HD uint8_t tatp_type(const uint8_t* r, int i) { return r[(size_t)i * TM + 1]; }
 TXN_HD uint32_t tatp_ver(const TMsg& m) { return get32(m.b + 51); }
+// A lock refused by a holder of the same key aborts the transaction exactly as one refused through false sharing does.
+// (The reference's client_lock.cc:741-749 leaves kRejectLockSameKey out of its final reply types and re-sends the lock
+// message as a kRead: SURVEY.md, appendix of quirks.  That is not reproduced.)
+TXN_HD bool tatp_lock_refused(uint8_t type) { return type == T_REJECT_LOCK || type == T_REJECT_LOCK_SAME_KEY; }
 
 // r: the replies to the client's records of the last tatp_emit, in the same order
 template <class Sink>
@@ -304,6 +310,7 @@ TXN_HD void tatp_absorb(const Cfg& w, TatpClient& c, const uint8_t* r, Sink& sin
         case 0:
           tatp_load(c.a, r, 0); tatp_load(c.b, r, 1); tatp_load(c.c, r, 2); tatp_load(c.d, r, 3);
           c.lock_a = tatp_type(r, 1) == T_GRANT_LOCK; c.lock_b = tatp_type(r, 3) == T_GRANT_LOCK;
+          sink.lock_reply(tatp_type(r, 1)); sink.lock_reply(tatp_type(r, 3));   // client_lock.cc:718 lock_cnt += 2
           if (tatp_type(r, 2) == T_NOT_EXIST || !c.lock_a || !c.lock_b) {      // :400-420
             if (c.lock_a) c.phase = 1; else if (c.lock_b) c.phase = 2; else tatp_finish(w, c, false, sink);
           } else {
@@ -332,7 +339,8 @@ TXN_HD void tatp_absorb(const Cfg& w, TatpClient& c, const uint8_t* r, Sink& sin
         case 0: c.phase = 1; break;
         case 1:
           tatp_load(c.a, r, 0); tatp_load(c.b, r, 1);
-          if (tatp_type(r, 1) == T_REJECT_LOCK) tatp_finish(w, c, false, sink);   // :642
+          sink.lock_reply(tatp_type(r, 1));
+          if (tatp_lock_refused(tatp_type(r, 1))) tatp_finish(w, c, false, sink);   // :642
           else { memcpy(c.a.b + 11 + 36, &c.vlr, 4); c.phase = 2; }        // sub_val->vlr_location (:646)
           break;
         case 2:
@@ -351,7 +359,8 @@ TXN_HD void tatp_absorb(const Cfg& w, TatpClient& c, const uint8_t* r, Sink& sin
         case 1: tatp_load(c.c, r, 0); if (tatp_type(r, 0) == T_NOT_EXIST) tatp_finish(w, c, false, sink); else c.phase = 2; break;   // :781
         case 2:
           tatp_load(c.a, r, 0); tatp_load(c.b, r, 1);
-          if (tatp_type(r, 0) == T_GRANT_READ || tatp_type(r, 1) == T_REJECT_LOCK) {   // :831-841: row exists or lock refused
+          sink.lock_reply(tatp_type(r, 1));
+          if (tatp_type(r, 0) == T_GRANT_READ || tatp_lock_refused(tatp_type(r, 1))) {   // :831-841: row exists or lock refused
             if (tatp_type(r, 1) == T_GRANT_LOCK) c.phase = 3; else tatp_finish(w, c, false, sink);
           } else {
             c.a.b[11 + 1] = 101;                                           // numberx[0] = magic (:846)
@@ -374,7 +383,8 @@ TXN_HD void tatp_absorb(const Cfg& w, TatpClient& c, const uint8_t* r, Sink& sin
         case 0: c.phase = 1; break;
         case 1:
           tatp_load(c.a, r, 0); tatp_load(c.b, r, 1);
-          if (tatp_type(r, 0) == T_NOT_EXIST || tatp_type(r, 1) == T_REJECT_LOCK) {   // :1024-1033
+          sink.lock_reply(tatp_type(r, 1));
+          if (tatp_type(r, 0) == T_NOT_EXIST || tatp_lock_refused(tatp_type(r, 1))) {   // :1024-1033
             if (tatp_type(r, 1) == T_GRANT_LOCK) c.phase = 2; else tatp_finish(w, c, false, sink);
           } else c.phase = 3;
           break;
@@ -572,30 +582,35 @@ struct DevClients {
   uint32_t* off;              // [n] offset of the client's first record in the round (= of its first reply)
   uint32_t* tile_sum;         // [tiles] records per tile; k_txn_scan turns it into the tiles' base offsets
   uint32_t* owner_cnt;        // [8] records of this round per destination shard
-  unsigned long long* stats;  // [0, 7) transactions started per type, [7, 14) committed per type
+  unsigned long long* stats;  // [0, 7) transactions started per type, [7, 14) committed per type, [14, 17) lock replies
+                              // absorbed, of them kRejectLock, kRejectLockSameKey
   uint8_t* req;               // the round, contiguous in client order
   uint8_t* dst;
   uint32_t* pub;              // mapped pinned host block: [0] records of the round, [1 + o] of them for shard o
 };
 
-// one absorb starts at most one transaction and commits at most one
+constexpr uint32_t kDevStats = 17;   // words of DevClients::stats
+
+// one absorb starts at most one transaction, commits at most one and sees at most two lock replies
 struct DevSink {
   int began, done;
+  uint32_t lock[3];             // lock replies, of them kRejectLock, kRejectLockSameKey
   __host__ __device__ void begin(uint8_t t) { began = t; }
   __host__ __device__ void commit(uint8_t t) { done = t; }
+  __host__ __device__ void lock_reply(uint8_t t) { lock[0]++; lock[1] += t == T_REJECT_LOCK; lock[2] += t == T_REJECT_LOCK_SAME_KEY; }
 };
 
 template <int KIND>           // DINT_TATP (4) or DINT_SMALLBANK (5)
 __global__ void __launch_bounds__(dint::kThreads, 1) k_txn_step(const DevClients d, const uint8_t* resp, int first) {
   constexpr uint32_t MSG = KIND == 4 ? TM : SMSZ;
-  __shared__ uint32_t s_stats[14], s_own[8], s_sum;
-  if (threadIdx.x < 14) s_stats[threadIdx.x] = 0;
+  __shared__ uint32_t s_stats[kDevStats], s_own[8], s_sum;
+  if (threadIdx.x < kDevStats) s_stats[threadIdx.x] = 0;
   if (threadIdx.x < 8) s_own[threadIdx.x] = 0;
   if (threadIdx.x == 0) s_sum = 0;
   __syncthreads();
   const uint32_t id = blockIdx.x * dint::kThreads + threadIdx.x;
   if (id < d.n) {
-    DevSink sink{-1, -1};
+    DevSink sink{-1, -1, {0, 0, 0}};
     Out o{d.stg + (size_t)id * kMaxRecords * MSG, d.stg_dst + (size_t)id * kMaxRecords, 0, 0, MSG};
     if constexpr (KIND == 4) {
       TatpClient& c = ((TatpClient*)d.cl)[id];
@@ -613,9 +628,10 @@ __global__ void __launch_bounds__(dint::kThreads, 1) k_txn_step(const DevClients
     atomicAdd(&s_sum, o.n);
     if (sink.began >= 0) atomicAdd(&s_stats[sink.began], 1u);
     if (sink.done >= 0) atomicAdd(&s_stats[7 + sink.done], 1u);
+    for (int i = 0; i < 3; i++) if (sink.lock[i]) atomicAdd(&s_stats[14 + i], sink.lock[i]);
   }
   __syncthreads();
-  if (threadIdx.x < 14 && s_stats[threadIdx.x]) atomicAdd(&d.stats[threadIdx.x], (unsigned long long)s_stats[threadIdx.x]);
+  if (threadIdx.x < kDevStats && s_stats[threadIdx.x]) atomicAdd(&d.stats[threadIdx.x], (unsigned long long)s_stats[threadIdx.x]);
   if (threadIdx.x < 8 && s_own[threadIdx.x]) atomicAdd(&d.owner_cnt[threadIdx.x], s_own[threadIdx.x]);
   if (threadIdx.x == 0) d.tile_sum[blockIdx.x] = s_sum;
 }

@@ -21,9 +21,12 @@ struct dint_txn {
   std::vector<SbClient> sc;
   uint64_t st_requests = 0, st_txns = 0, st_committed = 0, st_rounds = 0;
   uint64_t st_by_type[8] = {0}, st_commit_by_type[8] = {0};
+  uint64_t st_lock[3] = {0};   // lock replies absorbed, of them kRejectLock, kRejectLockSameKey (client_lock.cc's lock_cnt,
+                               // reject_sharing_cnt, reject_same_key_cnt)
 
   void begin(uint8_t type) { st_txns++; st_by_type[type]++; }          // the Sink of the shared state machines
   void commit(uint8_t type) { st_committed++; st_commit_by_type[type]++; }
+  void lock_reply(uint8_t type) { st_lock[0]++; st_lock[1] += type == T_REJECT_LOCK; st_lock[2] += type == T_REJECT_LOCK_SAME_KEY; }
 };
 
 extern "C" {
@@ -76,6 +79,11 @@ void dint_txn_feed(dint_txn* w, const void* resp) {
 void dint_txn_stats(const dint_txn* w, uint64_t out[18]) {
   out[0] = w->st_requests; out[1] = w->st_txns; out[2] = w->st_committed; out[3] = w->st_rounds;
   for (int i = 0; i < 7; i++) { out[4 + i] = w->st_by_type[i]; out[11 + i] = w->st_commit_by_type[i]; }
+}
+// out: kAcquireLock replies absorbed, of them refused through false sharing (kRejectLock) and by a holder of the same
+// key (kRejectLockSameKey): the counters behind tatp/caladan/client_lock.cc:403-428.  smallbank: zeros.
+void dint_txn_lock_stats(const dint_txn* w, uint64_t out[3]) {
+  for (int i = 0; i < 3; i++) out[i] = w->st_lock[i];
 }
 
 }  // extern "C"

@@ -30,7 +30,11 @@
 //
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
-//                        [--linger-us U] [--populate N] [--mon-port 20231]
+//                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
+//
+// --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
+// the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
+// server answers (tatp/ebpf/lock_kern.c:289-298); a client that speaks tatp/caladan/proto.h counts the two apart.
 //
 // --mon-port P: the reference servers' utilisation channel (tatp/udp/server_shard.cc:213-274: a thread samples the CPU
 // time of the server's cores once a second, another answers any datagram on UDP :20231 with `struct {double ucores;
@@ -106,7 +110,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -118,8 +122,11 @@ int main(int argc, char** argv) {
   if (n_sock > 8) n_sock = 8;                         // the reference runs `server 8` (exp/run_lock_fasst.sh)
   std::string bind_addr = "0.0.0.0";
   std::vector<int> devices;
-  for (int i = 2; i + 1 < argc; i += 2) {
+  bool holder_keys = false;
+  for (int i = 2; i < argc; i += 2) {
     const std::string a = argv[i];
+    if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the one option without a value
+    if (i + 1 >= argc) break;
     const char* v = argv[i + 1];
     if (a == "--port") port = atoi(v);
     else if (a == "--bind") bind_addr = v;
@@ -149,6 +156,7 @@ int main(int argc, char** argv) {
   // ---- engine: the state the reference keeps in its global arrays lives on the GPU(s) ----
   dint_cfg cfg;
   dint_default_cfg(kind, &cfg);                       // kLockHashSize, table sizes, ring length of the reference
+  if (holder_keys) cfg.flags |= DINT_CFG_LOCK_HOLDER_KEYS;   // dint_create refuses it for a kind other than tatp
   if (populate >= 0) { cfg.subs_populate = (uint32_t)populate; cfg.accts_populate = (uint32_t)populate; }   // a prefix of the reference's population
   dint_engine* eng = nullptr;
   dint_cluster* cluster = nullptr;

@@ -13,6 +13,9 @@ from . import _build
 from .wire import MSG_SIZE, LOG_ENTRY_SIZE, KIND_NAMES
 
 DINT_OK, DINT_EPROTO = 0, -71
+# dint_cfg.flags bit (tatp): keep the holder's key beside every lock bit, so that a refused kAcquireLock is answered
+# kRejectLockSameKey (28) or kRejectLock (8, false sharing) as tatp/ebpf/lock_kern.c:289-298 does
+DINT_CFG_LOCK_HOLDER_KEYS = 1
 
 
 class DintCfg(C.Structure):
@@ -56,7 +59,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -114,6 +117,7 @@ def lib():
     L.dint_txn_clients_stats.restype = i32; L.dint_txn_clients_stats.argtypes = [vp, C.POINTER(u64)]
     L.dint_txn_clients_peek.restype = i32; L.dint_txn_clients_peek.argtypes = [vp, vp, vp, C.POINTER(u64), vp, C.POINTER(u64)]
     L.dint_txn_clients_times.restype = i32; L.dint_txn_clients_times.argtypes = [vp, C.POINTER(C.c_double)]
+    L.dint_txn_clients_lock_stats.restype = i32; L.dint_txn_clients_lock_stats.argtypes = [vp, C.POINTER(u64)]
     L.dint_txn_clients_destroy.restype = None; L.dint_txn_clients_destroy.argtypes = [vp]
     L.dint_cluster_clients_create.restype = i32; L.dint_cluster_clients_create.argtypes = [vp, C.POINTER(DintClientsCfg), C.POINTER(vp)]
     L.dint_cluster_clients_run.restype = i32; L.dint_cluster_clients_run.argtypes = [vp, u32]
@@ -132,6 +136,7 @@ def lib():
     L.dint_kv_get.restype = i32; L.dint_kv_get.argtypes = [vp, i32, u64, vp, C.POINTER(u32)]
     L.dint_kv_count.restype = C.c_int64; L.dint_kv_count.argtypes = [vp, i32]
     L.dint_lock_state.restype = i32; L.dint_lock_state.argtypes = [vp, i32, u32, C.POINTER(u32)]
+    L.dint_lock_holder.restype = i32; L.dint_lock_holder.argtypes = [vp, i32, u32, C.POINTER(u64)]
     L.dint_lock_slot.restype = u32; L.dint_lock_slot.argtypes = [vp, i32, u64]
     L.dint_dump_log.restype = i32; L.dint_dump_log.argtypes = [vp, vp, C.POINTER(u64)]
     L.dint_log_entry_size.restype = u32; L.dint_log_entry_size.argtypes = [i32]
@@ -156,12 +161,16 @@ class DintError(RuntimeError):
 
 
 def default_cfg(kind, **over):
+    """dint_default_cfg() with fields overridden by name; lock_holder_keys=True sets DINT_CFG_LOCK_HOLDER_KEYS."""
     cfg = DintCfg()
     lib().dint_default_cfg(kind, C.byref(cfg))
     for k, v in over.items():
         if k == "kv_capacity_log2":
             for i, x in enumerate(v):
                 cfg.kv_capacity_log2[i] = x
+        elif k == "lock_holder_keys":
+            if v:
+                cfg.flags |= DINT_CFG_LOCK_HOLDER_KEYS
         else:
             setattr(cfg, k, v)
     return cfg
@@ -397,6 +406,15 @@ class Engine:
             raise DintError(rc, "dint_lock_state")
         return out[0], out[1]
 
+    def lock_holder(self, table, slot):
+        """tatp with lock_holder_keys: the key the last granted kAcquireLock left in the slot (stale once the slot is
+        free)."""
+        out = C.c_uint64(0)
+        rc = lib().dint_lock_holder(self.h, table, slot, C.byref(out))
+        if rc != 0:
+            raise DintError(rc, "dint_lock_holder")
+        return out.value
+
     def dump_log(self):
         es = LOG_ENTRY_SIZE[self.kind]
         n = self.cfg.log_ring
@@ -589,6 +607,14 @@ class GpuTxnClients:
         d["by_type"] = {n: (int(out[4 + i]), int(out[11 + i])) for i, n in enumerate(names)}
         d["fallback_rounds"] = int(out[18])
         return d
+
+    def lock_stats(self):
+        """TxnWorkload.lock_stats()'s dict, counted on the devices."""
+        out = (C.c_uint64 * 3)()
+        rc = lib().dint_txn_clients_lock_stats(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_lock_stats")
+        return {"locks": int(out[0]), "reject_sharing": int(out[1]), "reject_same_key": int(out[2])}
 
     def peek(self):
         """(next_req, next_dst, last_resp) in global client order: the pending round's requests and destination

@@ -34,6 +34,7 @@ def lib():
         L.dint_txn_next.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.dint_txn_feed.argtypes = [C.c_void_p, C.c_void_p]
         L.dint_txn_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.dint_txn_lock_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
         _lib = L
     return _lib
 
@@ -81,6 +82,14 @@ class TxnWorkload:
         names = TATP_TXN_NAMES if self.kind == TATP else SMALLBANK_TXN_NAMES
         d["by_type"] = {n: (int(out[4 + i]), int(out[11 + i])) for i, n in enumerate(names)}
         return d
+
+    def lock_stats(self):
+        """The lock counters of tatp/caladan/client_lock.cc: kAcquireLock replies absorbed, and how many of them were
+        refused through false sharing (kRejectLock: another key holds the slot) and by a holder of the same key
+        (kRejectLockSameKey, sent only by servers created with lock_holder_keys).  smallbank: zeros."""
+        out = (C.c_uint64 * 3)()
+        lib().dint_txn_lock_stats(self.h, out)
+        return {"locks": int(out[0]), "reject_sharing": int(out[1]), "reject_same_key": int(out[2])}
 
 
 def partition_by_shard(req, dst, n_shards, msg):

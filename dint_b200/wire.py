@@ -47,6 +47,9 @@ class Tatp:               # tatp/udp/net.h:15-52
      kAbortAck, kCommitAck, kRejectCommit, kCommitPrim, kCommitBck, kCommitLog, kCommitPrimAck,
      kCommitBckAck, kCommitLogAck, kInsertPrim, kInsertBck, kInsertPrimAck, kInsertBckAck, kDeletePrim,
      kDeleteBck, kDeleteLog, kDeletePrimAck, kDeleteBckAck, kDeleteLogAck) = range(28)
+    # reply of the eBPF lock server (tatp/ebpf/utils.h:73, tatp/caladan/proto.h:52): the refused lock is held for the
+    # same key; kRejectLock then means false sharing.  Sent only by engines created with lock_holder_keys.
+    kRejectLockSameKey = 28
     kSubscriber, kSecondSubscriber, kAccessInfo, kSpecialFacility, kCallForwarding = range(5)
 
 

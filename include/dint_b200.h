@@ -68,7 +68,7 @@ typedef struct dint_cfg {
   uint32_t shard_id;
   uint32_t chunk;          /* requests per internal launch group (0 = default 1<<20) */
   uint32_t kv_capacity_log2[5]; /* per-table open-addressing capacity (0 = auto: >= 2x expected keys) */
-  uint32_t flags;          /* reserved, must be 0 */
+  uint32_t flags;          /* DINT_CFG_* option bits (below); the other bits are reserved */
   uint32_t txn_shards;     /* tatp / smallbank replica placement (tatp/caladan/client_udp_shard.cc:187,490-531 generalised
                               from 3 to G shards): 0 or 1 = this server holds every key (the reference: all three
                               shards populate everything); G > 3: dint_populate() keeps only keys whose primary
@@ -76,6 +76,18 @@ typedef struct dint_cfg {
   uint32_t txn_shard_id;
   uint32_t reserved[2];
 } dint_cfg;
+
+/*
+ * dint_cfg.flags bit 0, tatp only (dint_create / dint_cluster_create answer DINT_EINVAL for another kind): keep the
+ * HOLDER'S KEY beside every lock bit, as the reference's eBPF lock server does (tatp/ebpf/lock_kern.c:12-16 `struct
+ * txn_lock {u64 lock_bit; u64 key}`, written by a granted kAcquireLock, :292).  A refused kAcquireLock is then answered
+ * kRejectLockSameKey (28) when the holder's key equals the request's -- a true conflict -- and kRejectLock (8) when it
+ * differs -- false sharing: two keys hashed to one lock slot (lock_kern.c:289-298, tatp/ebpf/utils.h:73,
+ * tatp/caladan/proto.h:52).  Releases leave the word alone, as the reference does (lock_kern.c:338,423,609,1119,1196);
+ * it means something only while the bit is set.  Costs one u64 per lock slot (896 MB at the reference's sizes).
+ * Without the bit nothing is allocated and every refused acquire is answered 8, as tatp/udp/server_shard.cc:123-132.
+ */
+#define DINT_CFG_LOCK_HOLDER_KEYS 1u
 
 typedef struct dint_engine dint_engine;
 
@@ -254,6 +266,9 @@ int dint_kv_get(dint_engine *e, int table, uint64_t key, void *val, uint32_t *ve
 int64_t dint_kv_count(dint_engine *e, int table);
 /* lock_2pl: out = {num_ex, num_sh}; lock_fasst: {lock, ver}; tatp: {lock, 0}; smallbank: {num_ex, num_sh} */
 int dint_lock_state(dint_engine *e, int table, uint32_t slot, uint32_t out[2]);
+/* tatp with DINT_CFG_LOCK_HOLDER_KEYS: the key the last granted kAcquireLock left in the slot (tatp/ebpf/lock_kern.c:292;
+ * 0 = never granted; stale once dint_lock_state says the slot is free).  DINT_EINVAL without the option. */
+int dint_lock_holder(dint_engine *e, int table, uint32_t slot, uint64_t *key);
 /* slot the reference would compute for a lock id / key (fasthash64 % size) -- for tests */
 uint32_t dint_lock_slot(dint_engine *e, int table, uint64_t key_or_lid);
 /* copies ring 0 of the commit log (log_ring entries of dint_log_entry_size bytes, laid out as the
@@ -337,6 +352,13 @@ int dint_txn_clients_run(dint_txn_clients *t, uint32_t rounds);
 int dint_txn_clients_stats(dint_txn_clients *t, uint64_t out[19]);
 int dint_txn_clients_peek(dint_txn_clients *t, void *next_req, uint8_t *next_dst, uint64_t *n_next, void *last_resp, uint64_t *n_last);
 int dint_txn_clients_times(dint_txn_clients *t, double out[3]);
+/* The lock counters of tatp/caladan/client_lock.cc, summed over the clients (synchronises): [0] kAcquireLock replies
+ * absorbed (lock_cnt, :718,1056,1309,1583), [1] of them kRejectLock = refused through false sharing
+ * (reject_sharing_cnt), [2] kRejectLockSameKey = refused by a holder of the same key (reject_same_key_cnt); the two
+ * ratios [1]/[0] and [2]/[0] are what the reference prints (:403-428,449-462).  [2] stays 0 against servers without
+ * DINT_CFG_LOCK_HOLDER_KEYS; smallbank: all 0 (S/X counters have no single holder, and no such wire type).  The host
+ * clients of libdint_wl.so count the same three words. */
+int dint_txn_clients_lock_stats(dint_txn_clients *t, uint64_t out[3]);
 void dint_txn_clients_destroy(dint_txn_clients *t);
 
 /*
