@@ -38,6 +38,10 @@ static const uint32_t kMsgSize[DINT_NUM_KINDS] = {6, 9, 53, 53, 55, 23};
 static const uint32_t kLogEntry[DINT_NUM_KINDS] = {0, 0, 56, 0, 64, 32};
 static const uint32_t kValSize[DINT_NUM_KINDS] = {0, 0, 0, 40, 40, 8};
 
+// Kernel kind of a store engine with the eBPF cache tier: not a public dint_kind, so the store's own kernels are
+// instantiated exactly as before and the tier's only when an engine asks for it (see exec_kind).
+constexpr int kExecStoreEbpf = DINT_NUM_KINDS;
+
 // The one place where an engine's run-time kind picks the kernel templates: calls f(std::integral_constant<int, K>{})
 // and returns what f returns.  Record-size-keyed kernels are instantiated with Wire<K>::MSG.
 template <class F>
@@ -49,6 +53,7 @@ static int with_kind(int kind, F&& f) {
     case DINT_STORE: return f(std::integral_constant<int, K_STORE>{});
     case DINT_TATP: return f(std::integral_constant<int, K_TATP>{});
     case DINT_SMALLBANK: return f(std::integral_constant<int, K_SMALLBANK>{});
+    case kExecStoreEbpf: return f(std::integral_constant<int, K_STORE_EBPF>{});
   }
   return set_err(DINT_EINVAL, "bad kind");
 }
@@ -137,6 +142,9 @@ struct dint_engine {
   // KV host mirrors
   KvHost kv[kMaxTables];
 };
+
+// the kind whose kernels serve this engine: its public kind, or the store's cache-tier kind
+static int exec_kind(const dint_engine* e) { return e->ctx.ecache ? kExecStoreEbpf : e->kind; }
 
 template <typename T>
 static int dalloc(dint_engine* e, T** p, size_t count, bool zero = true) {
@@ -248,7 +256,7 @@ static int launch_chunk_t(dint_engine* e, const Ctx& c, cudaStream_t s) {
 }
 
 static int launch_chunk(dint_engine* e, const Ctx& c, cudaStream_t s) {
-  return with_kind(e->kind, [&](auto k) { return launch_chunk_t<decltype(k)::value>(e, c, s); });
+  return with_kind(exec_kind(e), [&](auto k) { return launch_chunk_t<decltype(k)::value>(e, c, s); });
 }
 
 template <int KIND>
@@ -369,9 +377,9 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
     N.entries = (uint8_t*)fresh;
     {
       ProfScope ps(e, s, KT_LOAD);
-      with_kind(e->kind, [&](auto k) {
+      with_kind(exec_kind(e), [&](auto k) {
         constexpr int K = decltype(k)::value;
-        if constexpr (K == K_STORE || K == K_TATP || K == K_SMALLBANK) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
+        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
         return DINT_OK;
       });
     }
@@ -645,6 +653,12 @@ static int create_impl(dint_engine* e) {
   // holder keys: plain HBM, outside the persisting window below -- only lock requests touch them, and the window is
   // for what every request touches
   if ((cf.flags & DINT_CFG_LOCK_HOLDER_KEYS) && (rc = dalloc(e, &c.holder, groups))) return rc;
+  // the eBPF store's cache sets, one per bucket (store/ebpf/store_kern.c:25-30): plain HBM, zeroed = every slot invalid
+  if (cf.flags & DINT_CFG_STORE_EBPF_MASK) {
+    c.ecache_variant = (cf.flags & DINT_CFG_STORE_EBPF_MASK) >> 1;
+    if ((rc = dalloc(e, &c.ecache, groups * kEcSetBytes))) return rc;
+    if ((rc = dalloc(e, &c.ecache_stats, EC_NSTATS))) return rc;
+  }
   {
     uint32_t fl = 25;                                  // 2^25 nibbles = 16 MB per set: L2-resident
     while (fl > 10 && (1ULL << (fl - 1)) >= groups * 2 + 2048) fl--;   // tiny group spaces need less
@@ -706,7 +720,7 @@ static int create_impl(dint_engine* e) {
   if ((rc = dalloc(e, &c.counters, kNumCounters))) return rc;
   if ((rc = dalloc(e, &c.gbar, 4))) return rc;
 
-  if ((rc = with_kind(e->kind, [&](auto k) { return grids_for<decltype(k)::value>(e); }))) return rc;
+  if ((rc = with_kind(exec_kind(e), [&](auto k) { return grids_for<decltype(k)::value>(e); }))) return rc;
   int coop = 0;
   CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, e->device));
   if (!coop) return set_err(DINT_ENODEV, "device lacks cooperative launch");
@@ -732,6 +746,7 @@ int dint_create(int kind, const dint_cfg* cfg, int device, dint_engine** out) {
   if (cf.n_shards == 0) cf.n_shards = 1;
   if (cf.shard_id >= cf.n_shards || cf.lock_slots == 0) { delete e; return set_err(DINT_EINVAL, "bad shard/lock_slots"); }
   if ((cf.flags & DINT_CFG_LOCK_HOLDER_KEYS) && kind != DINT_TATP) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_LOCK_HOLDER_KEYS is a tatp option"); }
+  if ((cf.flags & DINT_CFG_STORE_EBPF_MASK) && kind != DINT_STORE) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_STORE_EBPF_* is a store option"); }
   if (cf.chunk == 0) cf.chunk = 1u << 20;
   e->chunk = (cf.chunk + kTile - 1) / kTile * kTile;
   {
@@ -757,7 +772,7 @@ int dint_route_owner(dint_engine* e, const void* req_dev, uint64_t n, uint8_t* o
   const uint32_t blocks = (uint32_t)((n + kThreads - 1) / kThreads);
   const uint8_t* rq = (const uint8_t*)req_dev;
   e->stats.kernel_launches++;
-  with_kind(e->kind, [&](auto k) {
+  with_kind(exec_kind(e), [&](auto k) {
     k_route_owner<decltype(k)::value><<<blocks, kThreads, 0, s>>>(e->ctx, rq, (uint32_t)n, owner_dev);
     return DINT_OK;
   });
@@ -784,7 +799,7 @@ int dint_route_partition(dint_engine* e, const void* req_dev, const uint8_t* own
   k_exact_scan<<<n_shards, kThreads, 0, s>>>(tilecnt, tiles, totals);
   const uint8_t* rq = (const uint8_t*)req_dev;
   uint8_t* out = (uint8_t*)sorted_dev;
-  with_kind(e->kind, [&](auto k) {
+  with_kind(exec_kind(e), [&](auto k) {
     k_exact_scatter<Wire<decltype(k)::value>::MSG><<<tiles, kThreads, 0, s>>>(rq, owner_dev, (uint32_t)n, n_shards, tilecnt, totals, out, perm_dev);
     return DINT_OK;
   });
@@ -819,7 +834,7 @@ int dint_route_dispatch(dint_engine* e, const void* req_dev, const uint8_t* owne
   for (uint32_t i = 0; i < kMaxShards; i++) { a.slab.p[i] = slab_ptrs->p[i]; a.sig.p[i] = sig_ptrs ? sig_ptrs->p[i] : 0; }
   cudaStream_t s = (cudaStream_t)cuda_stream;
   e->stats.kernel_launches += 1;
-  return with_kind(e->kind, [&](auto k) { return route_dispatch_t<decltype(k)::value>(e, a, s); });
+  return with_kind(exec_kind(e), [&](auto k) { return route_dispatch_t<decltype(k)::value>(e, a, s); });
 }
 
 int dint_route_combine(dint_engine* e, const dint_peer_ptrs* reply_slab_ptrs, const uint8_t* owner_dev, const uint32_t* tilebase_dev,
@@ -841,7 +856,7 @@ int dint_route_combine(dint_engine* e, const dint_peer_ptrs* reply_slab_ptrs, co
   for (uint32_t i = 0; i < kMaxShards; i++) a.slab.p[i] = reply_slab_ptrs->p[i];
   cudaStream_t s = (cudaStream_t)cuda_stream;
   e->stats.kernel_launches++;
-  return with_kind(e->kind, [&](auto k) { return route_combine_t<Wire<decltype(k)::value>::MSG>(e, a, s); });
+  return with_kind(exec_kind(e), [&](auto k) { return route_combine_t<Wire<decltype(k)::value>::MSG>(e, a, s); });
 }
 
 int dint_p2p_wait(dint_engine* e, const uint32_t* local_sig_dev, uint32_t n_shards, uint32_t epoch, uint32_t* flags_dev, void* cuda_stream) {
@@ -872,7 +887,7 @@ int dint_route_unpermute(dint_engine* e, const void* sorted_dev, const uint32_t*
   e->stats.kernel_launches++;
   const uint8_t* in = (const uint8_t*)sorted_dev;
   uint8_t* out = (uint8_t*)out_dev;
-  with_kind(e->kind, [&](auto k) {
+  with_kind(exec_kind(e), [&](auto k) {
     k_exact_unpermute<Wire<decltype(k)::value>::MSG><<<(uint32_t)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>(in, perm_dev, (uint32_t)n, out);
     return DINT_OK;
   });
@@ -976,6 +991,7 @@ static void snapshot_regions(dint_engine* e, std::vector<std::pair<void*, size_t
   if (e->kind == DINT_FASST) { r.push_back({c.ver, g * sizeof(uint32_t)}); r.push_back({c.lockbits, ((g + 31) / 32) * 4}); }
   if (e->kind == DINT_TATP) r.push_back({c.lockbits, ((g + 31) / 32) * 4});
   if (c.holder) r.push_back({c.holder, g * sizeof(uint64_t)});
+  if (c.ecache) r.push_back({c.ecache, g * kEcSetBytes});
   for (uint32_t t = 0; t < c.n_tables; t++) {
     r.push_back({c.tbl[t].entries, (size_t)(c.tbl[t].cap_mask + 1) << c.tbl[t].ent_shift});
     r.push_back({c.tbl[t].live, 16});
@@ -1129,9 +1145,36 @@ int dint_kernel_times(dint_engine* e, dint_kernel_time* out, int max_entries) {
 }
 
 // ---- KV entry points (store / tatp / smallbank) -------------------------------------------------------
+// With the eBPF cache tier a (key, value) pair enters as the client's kInsert would (store/caladan/client_ebpf.cc:137-180):
+// through the tier, so the cache sets, dirty bits and bloom words are the ones the reference server would hold.  Keys
+// of another shard's buckets are skipped, as k_kv_load skips them.
+static int ec_serve_inserts(dint_engine* e, const uint64_t* keys, const uint8_t* vals, uint64_t n) {
+  using W = Wire<K_STORE_EBPF>;
+  const Ctx& c = e->ctx;
+  const uint64_t batch = 1u << 20;
+  std::vector<uint8_t> buf((size_t)batch * W::MSG);
+  for (uint64_t off = 0; off < n;) {
+    uint64_t m = 0;
+    for (; off < n && m < batch; off++) {
+      const uint32_t g = fast_mod(fasthash64_u64(keys[off]), c.tbl[0].lock_mod);
+      if (g % c.n_shards != c.shard_id) continue;
+      uint8_t* r = buf.data() + (size_t)m++ * W::MSG;
+      memset(r, 0, W::MSG);
+      r[W::TYPE] = 2;                                   // kInsert, ver 0
+      memcpy(r + W::KEY, &keys[off], 8);
+      memcpy(r + W::VAL, vals + (size_t)off * W::VALSZ, W::VALSZ);
+    }
+    if (m == 0) continue;
+    int rc = dint_submit(e, buf.data(), m, buf.data());
+    if (rc) return rc;
+  }
+  return DINT_OK;
+}
+
 int dint_load(dint_engine* e, int table, const uint64_t* keys, const void* vals, uint64_t n) {
   if (!e || table < 0 || table >= (int)e->ctx.n_tables || (n && (!keys || !vals))) return set_err(DINT_EINVAL, "bad table/arguments");
   CU(cudaSetDevice(e->device));
+  if (e->ctx.ecache) return ec_serve_inserts(e, keys, (const uint8_t*)vals, n);
   const uint32_t vs = kValSize[e->kind];
   const uint64_t batch = 1u << 20;
   uint64_t* dk = nullptr;
@@ -1169,6 +1212,11 @@ int dint_load(dint_engine* e, int table, const uint64_t* keys, const void* vals,
 int dint_populate(dint_engine* e) {
   if (!e) return DINT_EINVAL;
   if (e->ctx.n_tables == 0) return DINT_OK;       // lock / log servers start from zeroed arrays
+  if (e->ctx.ecache) {                            // the eBPF store starts empty and is filled over the wire
+    return store_ebpf_populate(e->cfg, [&](int, const uint64_t* k, const void* v, uint64_t n) {
+      return ec_serve_inserts(e, k, (const uint8_t*)v, n);
+    });
+  }
   return kv_populate(e->kind, e->cfg, [&](int table, const uint64_t* k, const void* v, uint64_t n) {
     return dint_load(e, table, k, v, n);
   });
@@ -1179,6 +1227,35 @@ int dint_kv_get(dint_engine* e, int table, uint64_t key, void* val, uint32_t* ve
   CU(cudaSetDevice(e->device));
   CU(cudaDeviceSynchronize());
   return kv_host_get(e->ctx, table, key, kValSize[e->kind], val, ver);
+}
+
+int dint_store_cache_set(dint_engine* e, uint32_t bucket, void* out) {
+  if (!e || !out || !e->ctx.ecache) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
+  const Ctx& c = e->ctx;
+  if (bucket % c.n_shards != c.shard_id || bucket / c.n_shards >= e->total_groups) return set_err(DINT_EINVAL, "bucket of another shard");
+  CU(cudaSetDevice(e->device));
+  CU(cudaDeviceSynchronize());
+  uint8_t s[kEcSetBytes];
+  CU(cudaMemcpy(s, c.ecache + (size_t)(bucket / c.n_shards) * kEcSetBytes, sizeof s, cudaMemcpyDeviceToHost));
+  uint8_t* o = (uint8_t*)out;                      // struct cache_entry, store/ebpf/utils.h:58-66
+  memset(o, 0, DINT_STORE_CACHE_ENTRY_BYTES);
+  memcpy(o, s, 32);                                // key[4]
+  memcpy(o + 32, s + 64, 160);                     // val[4][40]
+  memcpy(o + 192, s + 32, 16);                     // ver[4]
+  for (int i = 0; i < 4; i++) {
+    o[208 + i] = (s[56] >> i) & 1;                 // valid[4]
+    o[212 + i] = (s[57] >> i) & 1;                 // dirty[4]
+  }
+  memcpy(o + 216, s + 48, 8);                      // bloom_filter; lock (+224) = 0
+  return DINT_OK;
+}
+
+int dint_store_cache_stats(dint_engine* e, uint64_t out[5]) {
+  if (!e || !out || !e->ctx.ecache) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
+  CU(cudaSetDevice(e->device));
+  CU(cudaDeviceSynchronize());
+  CU(cudaMemcpy(out, e->ctx.ecache_stats, EC_NSTATS * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  return DINT_OK;
 }
 
 int64_t dint_kv_count(dint_engine* e, int table) {
@@ -1560,6 +1637,7 @@ int dint_cluster_create(int kind, const dint_cfg* cfg, int n_gpus, const int* de
   const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
   if (by_dst && n_gpus == 2) return set_err(DINT_EINVAL, "tatp / smallbank placement needs 1 or >= 3 shards (primary + 2 backups)");
   if (cfg && (cfg->flags & DINT_CFG_LOCK_HOLDER_KEYS) && kind != DINT_TATP) return set_err(DINT_EINVAL, "DINT_CFG_LOCK_HOLDER_KEYS is a tatp option");
+  if (cfg && (cfg->flags & DINT_CFG_STORE_EBPF_MASK) && kind != DINT_STORE) return set_err(DINT_EINVAL, "DINT_CFG_STORE_EBPF_* is a store option");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_err(DINT_ENODEV, "no CUDA device: dint_b200 has no CPU fallback"); }
   dint_cluster* cl = new dint_cluster();

@@ -36,7 +36,8 @@
 
 namespace dint {
 
-enum Kind { K_LOCK2PL = 0, K_FASST = 1, K_LOG = 2, K_STORE = 3, K_TATP = 4, K_SMALLBANK = 5 };
+enum Kind { K_LOCK2PL = 0, K_FASST = 1, K_LOG = 2, K_STORE = 3, K_TATP = 4, K_SMALLBANK = 5,
+            K_STORE_EBPF = 6 };   // internal: a store engine created with a DINT_CFG_STORE_EBPF_* variant (kv.cuh)
 // the kinds whose requests append to a commit log (K1 counts the appends per tile, K1b turns them into ring ordinals)
 template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK;
 
@@ -68,6 +69,7 @@ template <> struct Wire<K_LOG> {       // log_server/udp/net.h:23-30 {u8 type; u
 template <> struct Wire<K_STORE> {     // store/udp/net.h:34-41 (same shape)
   static constexpr int MSG = 53, TYPE = 0, KEY = 1, VAL = 9, VER = 49, VALSZ = 40;
 };
+template <> struct Wire<K_STORE_EBPF> : Wire<K_STORE> {};   // store/ebpf/utils.h:40-45 (same shape)
 template <> struct Wire<K_TATP> {      // tatp/udp/net.h:57-65 {u8 ord; u8 type; u8 table; u64 key; u8 val[40]; u32 ver}
   static constexpr int MSG = 55, TYPE = 1, TABLE = 2, KEY = 3, VAL = 11, VER = 51, VALSZ = 40, LOGENT = 64;
 };
@@ -154,6 +156,11 @@ struct Ctx {
   const uint32_t* skip;           // multi-GPU step: non-zero = a slab overflowed, serve nothing more (see k_p2p_wait)
   uint32_t* log_src;              // tatp: [chunk] per append of the chunk, (request index << 1) | is kCommitLog (K2, when
                                   // the chunk appends more than ring_n), for k_log_vals
+  // store with the eBPF cache tier (DINT_CFG_STORE_EBPF_*): one 256-byte cache set per local group, the variant, and the
+  // tier's counters (hits, bloom negatives, served by the table, write-backs, installs).  Null / 0 without the option.
+  uint8_t* ecache;
+  uint32_t ecache_variant;
+  unsigned long long* ecache_stats;
 };
 
 // address of tile T's replies (T counted from the start of the batch) when the replies are segmented by source

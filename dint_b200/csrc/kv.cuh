@@ -21,6 +21,9 @@
 #pragma once
 #include <functional>
 #include "engine.cuh"
+#ifdef __CUDACC__
+#include <cooperative_groups.h>
+#endif
 
 namespace dint {
 
@@ -226,6 +229,218 @@ DINT_D void apply_one<K_STORE>(const Ctx& c, uint8_t* rec, const KeyInfo& ki, co
   } else {
     if (kv_insert_from<40>(c.tbl[0], ki.key, ki.h, rec + W::VAL)) rec[W::TYPE] = 8;                  // kInsertAck
     else mark_invalid<K_STORE>(c, rec);
+  }
+}
+
+// ============================ store, eBPF cache tier (DINT_CFG_STORE_EBPF_*) =======================
+// The reference's eBPF store server: an XDP program keeps a 4-slot cache set per bucket in front of the user-space
+// `kvs` (store/ebpf/store_kern.c:25-30, utils.h:58-66), answers hits and bloom negatives itself, passes misses to
+// user space (store_user.c:127-165) and installs the table's answer from a TC egress program (store_kern.c:302-373).
+// apply_one<K_STORE_EBPF> is that whole path for one request.  Variants: 1 = store_kern.c (write-back + bloom word),
+// 2 = store_wb_kern.c (write-back, no bloom), 3 = store_wt_kern.c + store_wt_user.c (write-through).
+// Cache set, 256 bytes: tag block {u64 key[4]; u32 ver[4]; u64 bloom; u8 valid_mask; u8 dirty_mask; pad} at +0 (one
+// 64-byte fetch decides hit / bloom / victim), u8 val[4][40] at +64.
+// Every request is a writer of its group (a READ miss installs and may write back), so two of one set in a chunk are
+// replayed in index order.  Every table access of a request concerns its own bucket: the requested key or a victim of
+// the same set.
+enum : uint32_t { EC_WB_BLOOM = 1, EC_WB = 2, EC_WT = 3 };
+constexpr uint32_t kEcSetBytes = 256;
+enum : uint32_t { EC_HIT = 0, EC_BLOOM_NEG = 1, EC_TABLE = 2, EC_WRITEBACK = 3, EC_INSTALL = 4, EC_NSTATS = 5 };
+
+template <> DINT_D TypeInfo type_info<K_STORE_EBPF>(const uint8_t* rec) {
+  if (rec[Wire<K_STORE_EBPF>::TYPE] <= 2) return TypeInfo{C_WA, false, false};   // kRead / kSet / kInsert
+  return TypeInfo{0, true, false};                                                // store_user.c:164
+}
+template <> DINT_D KeyInfo key_info<K_STORE_EBPF>(const Ctx& c, const uint8_t* rec) { return key_info<K_STORE>(c, rec); }
+template <> struct Pre<K_STORE_EBPF> { uint4 t[4]; };   // the set's tag block
+DINT_D uint8_t* ec_set(const Ctx& c, uint32_t g) { return c.ecache + (size_t)g * kEcSetBytes; }
+template <> DINT_D Pre<K_STORE_EBPF> prefetch<K_STORE_EBPF>(const Ctx& c, const uint8_t*, const KeyInfo& ki, const TypeInfo&) {
+  Pre<K_STORE_EBPF> p;
+  kv_load_entry<40>(ec_set(c, ki.grp), p.t);
+  return p;
+}
+template <>
+DINT_D Pre<K_STORE_EBPF> prefetch_coop<K_STORE_EBPF>(const Ctx& c, const uint8_t*, const KeyInfo& ki, const TypeInfo&, bool active) {
+  Pre<K_STORE_EBPF> p;
+  kv_prefetch_home_coop<40>(active ? ec_set(c, ki.grp) : nullptr, active, p.t);
+  return p;
+}
+// warp-aggregated counter bump: the lanes that arrive together are partitioned by counter, one atomic per partition
+DINT_D void ec_count(const Ctx& c, uint32_t which) {
+  namespace cg = cooperative_groups;
+  const cg::coalesced_group arrived = cg::coalesced_threads();
+  const cg::coalesced_group peers = cg::labeled_partition(arrived, which);
+  if (peers.thread_rank() == 0) atomicAdd(&c.ecache_stats[which], (unsigned long long)peers.size());
+}
+DINT_D void ec_load_val(const uint8_t* set, int i, uint32_t (&w)[10]) {
+  const uint2* p = (const uint2*)(set + 64 + 40 * i);
+#pragma unroll
+  for (int k = 0; k < 5; k++) { const uint2 q = __ldcg(p + k); w[2 * k] = q.x; w[2 * k + 1] = q.y; }
+}
+DINT_D void ec_store_val(uint8_t* set, int i, const uint32_t (&w)[10]) {
+  uint2* p = (uint2*)(set + 64 + 40 * i);
+#pragma unroll
+  for (int k = 0; k < 5; k++) p[k] = make_uint2(w[2 * k], w[2 * k + 1]);
+}
+// the table side (store/ebpf/kvs.h), each call probing afresh: earlier calls of the same request may have written
+DINT_D uint8_t* ec_tbl_find(const Ctx& c, uint64_t key, uint64_t h, uint4 (&v)[4]) {
+  kv_prefetch_home<40>(c, 0, h, v);
+  return kv_find<40>(c.tbl[0], key, h, v);
+}
+// false: the table is full (the reference's chained table never is) and the pair was lost
+DINT_D bool ec_set_evict(const Ctx& c, uint64_t key, const uint32_t (&w)[10], uint32_t ver) {   // kvs.h:103-121
+  uint4 v[4];
+  const uint64_t h = fasthash64_u64(key);
+  uint8_t* e = ec_tbl_find(c, key, h, v);
+  if (e) { kv_write_val<40>(e, w); *((uint32_t*)(e + 8)) = ver; return true; }
+  return kv_insert_words<40>(c.tbl[0], key, h, w);   // kvs_insert: version 0, not `ver`
+}
+
+template <>
+DINT_D void apply_one<K_STORE_EBPF>(const Ctx& c, uint8_t* rec, const KeyInfo& ki, const Pre<K_STORE_EBPF>& pf, unsigned long long,
+                                    bool) {
+  using W = Wire<K_STORE_EBPF>;
+  const uint8_t t = rec[W::TYPE];
+  const uint32_t var = c.ecache_variant;
+  const bool wt = var == EC_WT, bloom_on = var == EC_WB_BLOOM;
+  uint8_t* set = ec_set(c, ki.grp);
+  uint32_t tw[16];                                    // tag block words: key[4] (0..7), ver[4] (8..11), bloom (12..13), masks (14)
+#pragma unroll
+  for (int k = 0; k < 4; k++) { tw[4 * k] = pf.t[k].x; tw[4 * k + 1] = pf.t[k].y; tw[4 * k + 2] = pf.t[k].z; tw[4 * k + 3] = pf.t[k].w; }
+  uint32_t valid = tw[14] & 15u, dirty = (tw[14] >> 8) & 15u;
+  uint64_t bloom = ((uint64_t)tw[13] << 32) | tw[12];
+  const uint64_t bit = 1ull << (ki.h >> 58);          // bf_hash, store_kern.c:80
+  const uint64_t key = ki.key;
+  int hit = -1;                                       // :69-72
+#pragma unroll
+  for (int i = 3; i >= 0; i--)
+    if (((valid >> i) & 1u) && tw[2 * i] == (uint32_t)key && tw[2 * i + 1] == (uint32_t)(key >> 32)) hit = i;
+  // victim slot of a miss: first invalid, else (write-back variants) first clean, else 0 (:116-125; store_wt_kern.c:104-108)
+  int vic = 0;
+  {
+    const uint32_t inv = ~valid & 15u, cln = ~dirty & 15u;
+    if (inv) vic = __ffs(inv) - 1;
+    else if (!wt && cln) vic = __ffs(cln) - 1;
+  }
+  const bool evict = !wt && ((valid >> vic) & 1u) && ((dirty >> vic) & 1u);
+  uint32_t rw[10];                                    // the request's value
+  ld_words_unaligned<10>(rec + W::VAL, rw);
+  bool tags_changed = false;
+  bool stored = true;                                 // false: the table was full and a pair was lost (answered 0xFF)
+  auto put_slot = [&](int i, uint64_t k, uint32_t ver) {
+    tw[2 * i] = (uint32_t)k; tw[2 * i + 1] = (uint32_t)(k >> 32); tw[8 + i] = ver; tags_changed = true;
+  };
+  // store_user.c:135,146,158: kvs_set_evict of the victim, which travelled in ext_message.{key2,val2,ver2}.  `first` runs
+  // between reading the victim and writing it back (the insert path's kvs_insert of the new key, :157-158).
+  auto write_back = [&](auto&& first) {
+    uint32_t ow[10];
+    ec_load_val(set, vic, ow);
+    const uint64_t ok = ((uint64_t)tw[2 * vic + 1] << 32) | tw[2 * vic];
+    const uint32_t over = tw[8 + vic];
+    first();
+    stored &= ec_set_evict(c, ok, ow, over);
+    ec_count(c, EC_WRITEBACK);
+  };
+  uint4 v[4];
+  if (t == 2) {                                       // kInsert
+    if (wt) {                                         // store_wt_kern.c:165-176, store_wt_user.c: kvs_insert
+      const uint32_t inv = ~valid & 15u;
+      if (inv) {
+        const int i = __ffs(inv) - 1;
+        put_slot(i, key, ld_u32_unaligned(rec + W::VER));   // the client's version, while the table holds 0
+        ec_store_val(set, i, rw);
+        valid |= 1u << i; dirty &= ~(1u << i);
+        ec_count(c, EC_INSTALL);
+      }
+      stored &= kv_insert_words<40>(c.tbl[0], key, ki.h, rw);
+      ec_count(c, EC_TABLE);
+    } else {
+      if (bloom_on) bloom |= bit;                     // store_kern.c:238-239
+      if (evict) {                                    // :252-283, then store_user.c:155-161 and the TC INSERT_ACK path
+        write_back([&] { stored &= kv_insert_words<40>(c.tbl[0], key, ki.h, rw); });
+        ec_count(c, EC_TABLE);
+        dirty &= ~(1u << vic);
+      } else {                                        // :284-295: cached dirty, the table does not hold it yet
+        valid |= 1u << vic; dirty |= 1u << vic;
+      }
+      put_slot(vic, key, 0);
+      ec_store_val(set, vic, rw);
+      ec_count(c, EC_INSTALL);
+    }
+    rec[W::TYPE] = 8;                                 // kInsertAck, the request's key / val / ver echoed
+  } else if (hit >= 0 && (t == 0 || !wt)) {
+    ec_count(c, EC_HIT);
+    if (t == 0) {                                     // :74-86
+      uint32_t w[10];
+      ec_load_val(set, hit, w);
+      st_words_unaligned<10>(rec + W::VAL, w);
+      st_u32_unaligned(rec + W::VER, tw[8 + hit]);
+      rec[W::TYPE] = 3;                               // kGrantRead
+    } else {                                          // :157-172: the reply keeps the client's ver
+      ec_store_val(set, hit, rw);
+      tw[8 + hit]++; tags_changed = true;
+      dirty |= 1u << hit;
+      rec[W::TYPE] = 5;                               // kSetAck
+    }
+    if (bloom_on) bloom |= bit;
+  } else if (bloom_on && !(bloom & bit)) {            // :88-94, :174-180: the bloom word says absent
+    ec_count(c, EC_BLOOM_NEG);
+    rec[W::TYPE] = 7;                                 // kNotExist, ver echoed
+  } else {
+    // XDP_PASS to user space; ext_message.ver1 carries the eviction flag (write-back variants)
+    ec_count(c, EC_TABLE);
+    if (evict) write_back([] {});
+    if (t == 0) {                                     // store_user.c:133-142
+      uint8_t* e = ec_tbl_find(c, key, ki.h, v);
+      if (e) {
+        const uint32_t* flat = (const uint32_t*)v;
+        uint32_t w[10];
+#pragma unroll
+        for (int k = 0; k < 10; k++) w[k] = flat[4 + k];
+        st_words_unaligned<10>(rec + W::VAL, w);
+        st_u32_unaligned(rec + W::VER, v[0].z);
+        rec[W::TYPE] = 3;
+        put_slot(vic, key, v[0].z);                   // TC install, store_kern.c:325-342 (wt: dirty untouched, :223-235)
+        ec_store_val(set, vic, w);
+        valid |= 1u << vic;
+        if (!wt) dirty &= ~(1u << vic);
+        if (bloom_on) bloom |= bit;
+        ec_count(c, EC_INSTALL);
+      } else {
+        if (!wt) { st_u32_unaligned(rec + W::VER, evict ? 1u : 0u); dirty &= ~(1u << vic); }   // :128-133, TC :345-352
+        rec[W::TYPE] = 7;
+      }
+    } else {                                          // kSet, store_user.c:144-153 (kvs.h:54-73)
+      if (wt && hit >= 0) valid &= ~(1u << hit);      // store_wt_kern.c:132: invalidated, never re-installed by TC
+      uint8_t* e = ec_tbl_find(c, key, ki.h, v);
+      uint32_t nv = 0;
+      if (e) {
+        kv_write_val<40>(e, rw);
+        nv = v[0].z + 1;
+        *((uint32_t*)(e + 8)) = nv;
+      }
+      st_u32_unaligned(rec + W::VER, nv);
+      rec[W::TYPE] = nv != 0 ? 5 : 7;
+      if (!wt) {
+        if (nv != 0) {                                // TC install of the table's new version
+          put_slot(vic, key, nv);
+          ec_store_val(set, vic, rw);
+          valid |= 1u << vic;
+          if (bloom_on) bloom |= bit;
+          ec_count(c, EC_INSTALL);
+        }
+        dirty &= ~(1u << vic);
+      }
+    }
+  }
+  if (!stored) mark_invalid<K_STORE_EBPF>(c, rec);   // as apply_one<K_STORE> answers an insert into a full table
+  const uint32_t masks = valid | (dirty << 8);
+  if (tags_changed || masks != (tw[14] & 0xF0Fu) || bloom != (((uint64_t)tw[13] << 32) | tw[12])) {
+    uint4* tp = (uint4*)set;
+    tp[0] = make_uint4(tw[0], tw[1], tw[2], tw[3]);
+    tp[1] = make_uint4(tw[4], tw[5], tw[6], tw[7]);
+    tp[2] = make_uint4(tw[8], tw[9], tw[10], tw[11]);
+    tp[3] = make_uint4((uint32_t)bloom, (uint32_t)(bloom >> 32), masks, 0u);
   }
 }
 
@@ -715,5 +930,27 @@ inline int kv_populate(int kind, const dint_cfg& cf, std::function<int(int, cons
     return sf.rc ? sf.rc : cfw.rc;
   }
 }
+
+// The eBPF store's population: its client's kInsert stream (store/caladan/client_ebpf.cc:137-180), as ONE sequential
+// server sees it -- 600 populate threads (:282) in thread order, each over its slice of the subscribers with fastrand
+// restarting at 0xdeadbeef (:138).  Same keys and value bytes as kv_populate's store, in another order and other draws.
+inline int store_ebpf_populate(const dint_cfg& cf, std::function<int(int, const uint64_t*, const void*, uint64_t)> sink) {
+  KvBatch b(0, 40, sink, cf);
+  const uint32_t S = cf.subs_populate, threads = 600, slice = S / threads;
+  for (uint32_t w = 0; w < threads; w++) {
+    uint64_t seed = 0xdeadbeef;
+    const uint32_t lo = w * slice, hi = (w == threads - 1) ? S : (w + 1) * slice;
+    for (uint32_t s = lo; s < hi; s++)
+      for (uint64_t sf = 1; sf <= 4; sf++)
+        for (uint64_t st = 0; st <= 16; st += 8) {
+          uint8_t* v = b.add((uint64_t)s | (sf << 32) | (st << 40));
+          v[1] = 0x5a;                                       // numberx[0] = kValMagic
+          v[0] = (uint8_t)((kv_fastrand(&seed) % 24) + 1);   // end_time
+        }
+  }
+  b.flush();
+  return b.rc;
+}
+
 
 }  // namespace dint

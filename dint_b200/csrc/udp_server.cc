@@ -31,10 +31,16 @@
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
 //                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
+//                        [--store-ebpf wb-bloom|wb|wt]
 //
 // --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
 // the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
 // server answers (tatp/ebpf/lock_kern.c:289-298); a client that speaks tatp/caladan/proto.h counts the two apart.
+//
+// --store-ebpf V (store): DINT_CFG_STORE_EBPF_* -- answer as the reference's eBPF store server (store/ebpf/store_kern.c,
+// store_wb_kern.c, store_wt_kern.c for V = wb-bloom, wb, wt), with its per-bucket cache sets in front of the table; the
+// server starts empty and --populate N serves the eBPF client's kInsert stream for N subscribers
+// (store/caladan/client_ebpf.cc:137-180).
 //
 // --mon-port P: the reference servers' utilisation channel (tatp/udp/server_shard.cc:213-274: a thread samples the CPU
 // time of the server's cores once a second, another answers any datagram on UDP :20231 with `struct {double ucores;
@@ -110,7 +116,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -123,6 +129,7 @@ int main(int argc, char** argv) {
   std::string bind_addr = "0.0.0.0";
   std::vector<int> devices;
   bool holder_keys = false;
+  uint32_t store_ebpf = 0;
   for (int i = 2; i < argc; i += 2) {
     const std::string a = argv[i];
     if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the one option without a value
@@ -140,6 +147,13 @@ int main(int argc, char** argv) {
     else if (a == "--linger-us") linger_us = atoi(v);
     else if (a == "--populate") populate = atoi(v);
     else if (a == "--mon-port") mon_port = atoi(v);
+    else if (a == "--store-ebpf") {
+      const std::string w = v;
+      if (w == "wb-bloom") store_ebpf = DINT_CFG_STORE_EBPF_WB_BLOOM;
+      else if (w == "wb") store_ebpf = DINT_CFG_STORE_EBPF_WB;
+      else if (w == "wt") store_ebpf = DINT_CFG_STORE_EBPF_WT;
+      else { fprintf(stderr, "--store-ebpf takes wb-bloom, wb or wt\n"); return 2; }
+    }
     else { fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
   }
   if (batch_max < 1) batch_max = 1;
@@ -157,6 +171,7 @@ int main(int argc, char** argv) {
   dint_cfg cfg;
   dint_default_cfg(kind, &cfg);                       // kLockHashSize, table sizes, ring length of the reference
   if (holder_keys) cfg.flags |= DINT_CFG_LOCK_HOLDER_KEYS;   // dint_create refuses it for a kind other than tatp
+  cfg.flags |= store_ebpf;                                   // ... and this for a kind other than store
   if (populate >= 0) { cfg.subs_populate = (uint32_t)populate; cfg.accts_populate = (uint32_t)populate; }   // a prefix of the reference's population
   dint_engine* eng = nullptr;
   dint_cluster* cluster = nullptr;

@@ -42,6 +42,10 @@ class Store:              # store/udp/net.h:15-29
     kRead, kSet, kInsert, kGrantRead, kRejectRead, kSetAck, kRejectSet, kNotExist, kInsertAck, kRejectInsert = range(10)
 
 
+class StoreEbpf:          # store/ebpf/utils.h:21-32: the eBPF store server's packet types (the same values)
+    READ, SET, INSERT, GRANT_READ, REJECT_READ, SET_ACK, REJECT_SET, NOT_EXIST, INSERT_ACK, REJECT_INSERT = range(10)
+
+
 class Tatp:               # tatp/udp/net.h:15-52
     (kRead, kAcquireLock, kAbort, kCommit, kGrantRead, kRejectRead, kNotExist, kGrantLock, kRejectLock,
      kAbortAck, kCommitAck, kRejectCommit, kCommitPrim, kCommitBck, kCommitLog, kCommitPrimAck,

@@ -89,6 +89,40 @@ typedef struct dint_cfg {
  */
 #define DINT_CFG_LOCK_HOLDER_KEYS 1u
 
+/*
+ * dint_cfg.flags bits 1-2, store only (dint_create / dint_cluster_create answer DINT_EINVAL for another kind): answer as
+ * the reference's eBPF store server does instead of its UDP server (store/udp/server.cc).  The eBPF server keeps a 4-slot
+ * cache set per bucket in an XDP map (store/ebpf/store_kern.c:25-30, `struct cache_entry`, utils.h:58-66), answers hits
+ * there, passes misses to a user-space `kvs` (store_user.c:127-165) and installs the table's answer from a TC egress
+ * program (store_kern.c:302-373).  The tier leaks into the wire, so every reply depends on the hit / miss / eviction
+ * history and the cache is modelled exactly:
+ *   - a kSet that hits echoes the client's ver; one that misses returns the table's new version (store_user.c:148-149);
+ *   - a kRead of an absent key whose bloom bit is clear is answered kNotExist with the request's ver (store_kern.c:88-94);
+ *     a bloom false positive comes back kNotExist with ver = the eviction flag XDP put in ext_message.ver1 (:128-133);
+ *   - a miss takes the first invalid slot, else the first clean one, else slot 0 (:116-125); a dirty victim is written
+ *     back to the table first (kvs_set_evict, kvs.h:103-121), a clean one is overwritten;
+ *   - kInsert fills a slot in XDP (dirty, the table does not see it) or, over a dirty victim, also writes back and
+ *     inserts into the table (:226-297).  In the write-through variant (store_wt_kern.c:153-195) the cache keeps the
+ *     CLIENT'S version of an inserted key while the table holds 0, a kSet invalidates the cached copy, and nothing is
+ *     ever dirty.
+ * kReject* replies (a set locked by another server thread) are never produced, as with kRetry elsewhere; a type other
+ * than kRead / kSet / kInsert is answered 0xFF (DINT_EPROTO; store_user.c:164 panics).
+ * The server starts EMPTY: dint_populate serves the eBPF client's kInsert stream (store/caladan/client_ebpf.cc:137-180,
+ * 600 populate threads in thread order) through the tier, and dint_load serves its pairs as kInsert requests.
+ * Costs 256 bytes of HBM per bucket (2.3 GB at the reference's 9,000,000 buckets).  Without these bits nothing is
+ * allocated and the engine answers as store/udp/server.cc.
+ * Limit: a key that reaches the table by kvs_insert twice (a second kInsert of a key the table already holds) is kept
+ * twice by the reference's chained kvs (store/ebpf/kvs.h:75-101 never looks for an existing copy), which finds the copy
+ * in its newest chain entry first; the engine's open-addressing table keeps both too but finds the first-inserted one.
+ * Replies to such a key may then differ.  A key inserted once is served bit-exactly.  If the table is full (the
+ * reference's chained table never is) the request that could not store its pair is answered 0xFF (DINT_EPROTO).
+ */
+#define DINT_CFG_STORE_EBPF_WB_BLOOM (1u << 1)  /* store/ebpf/store_kern.c: write-back cache + 64-bit bloom word per set */
+#define DINT_CFG_STORE_EBPF_WB (2u << 1)        /* store/ebpf/store_wb_kern.c: write-back cache, no bloom word */
+#define DINT_CFG_STORE_EBPF_WT (3u << 1)        /* store/ebpf/store_wt_kern.c + store_wt_user.c: write-through cache */
+#define DINT_CFG_STORE_EBPF_MASK (3u << 1)
+#define DINT_STORE_CACHE_ENTRY_BYTES 232         /* sizeof(struct cache_entry), store/ebpf/utils.h:58-66 */
+
 typedef struct dint_engine dint_engine;
 
 /* Counters since create (or the last dint_reset_stats). */
@@ -263,6 +297,14 @@ int dint_sync(dint_engine *e);   /* waits for everything submitted on this engin
 /* ---- state inspection: parity of the final server state, not only of the wire ------------------ */
 /* kvs_get on the device table (store/udp/kvs.h:37-55): 0 = found, 1 = not found. */
 int dint_kv_get(dint_engine *e, int table, uint64_t key, void *val, uint32_t *ver);
+/* Cache set `bucket` (fasthash64(key) % 9,000,000 at the reference's sizes) of a store engine with the eBPF cache tier,
+ * written to `out` as the reference's struct cache_entry (232 bytes: key[4], val[4][40], ver[4], valid[4], dirty[4],
+ * bloom_filter, lock = 0).  DINT_EINVAL without the tier or for a bucket another shard owns. */
+int dint_store_cache_set(dint_engine *e, uint32_t bucket, void *out);
+/* The tier's counters since create: out[0] requests answered from the cache (hits), [1] bloom negatives, [2] requests
+ * served by the backing table (the user-space path), [3] dirty victims written back, [4] slots filled (installs and
+ * cached inserts). */
+int dint_store_cache_stats(dint_engine *e, uint64_t out[5]);
 int64_t dint_kv_count(dint_engine *e, int table);
 /* lock_2pl: out = {num_ex, num_sh}; lock_fasst: {lock, ver}; tatp: {lock, 0}; smallbank: {num_ex, num_sh} */
 int dint_lock_state(dint_engine *e, int table, uint32_t slot, uint32_t out[2]);
