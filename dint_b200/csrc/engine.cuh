@@ -37,9 +37,10 @@
 namespace dint {
 
 enum Kind { K_LOCK2PL = 0, K_FASST = 1, K_LOG = 2, K_STORE = 3, K_TATP = 4, K_SMALLBANK = 5,
-            K_STORE_EBPF = 6 };   // internal: a store engine created with a DINT_CFG_STORE_EBPF_* variant (kv.cuh)
+            K_STORE_EBPF = 6,     // internal: a store engine created with a DINT_CFG_STORE_EBPF_* variant (kv.cuh)
+            K_TATP_EBPF = 7 };    // internal: a tatp engine created with DINT_CFG_TATP_EBPF (kv.cuh)
 // the kinds whose requests append to a commit log (K1 counts the appends per tile, K1b turns them into ring ordinals)
-template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK;
+template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK || KIND == K_TATP_EBPF;
 
 constexpr int kTile = 128;       // wire records per tile = threads per CTA in K1/K2 (16 CTAs, i.e. 16 independent
                                  // latency chains, per SM)
@@ -73,6 +74,7 @@ template <> struct Wire<K_STORE_EBPF> : Wire<K_STORE> {};   // store/ebpf/utils.
 template <> struct Wire<K_TATP> {      // tatp/udp/net.h:57-65 {u8 ord; u8 type; u8 table; u64 key; u8 val[40]; u32 ver}
   static constexpr int MSG = 55, TYPE = 1, TABLE = 2, KEY = 3, VAL = 11, VER = 51, VALSZ = 40, LOGENT = 64;
 };
+template <> struct Wire<K_TATP_EBPF> : Wire<K_TATP> {};     // tatp/ebpf/utils.h:79-86 (same shape)
 template <> struct Wire<K_SMALLBANK> { // smallbank/udp/net.h:43-52 {u8 ord; u8 type; u8 table; u64 key; u8 val[8]; u32 ver}
   static constexpr int MSG = 23, TYPE = 1, TABLE = 2, KEY = 3, VAL = 11, VER = 19, VALSZ = 8, LOGENT = 32;
 };
@@ -161,6 +163,15 @@ struct Ctx {
   uint8_t* ecache;
   uint32_t ecache_variant;
   unsigned long long* ecache_stats;
+  // tatp with the eBPF cache tier (DINT_CFG_TATP_EBPF): `ecache` holds one cache set per bucket of every table and
+  // `ecache_stats` the tier's counters (EC_NSTATS_TATP); the chained tables are a {head, free list} pair per bucket
+  // (entry index + 1, 0 = none) over one pool of 256-byte chain entries with a bump allocator; tbkt_mod = the bucket
+  // count of each table.  Null / 0 without the option.
+  uint2* tchain;
+  uint8_t* tpool;
+  uint32_t* tpool_top;
+  uint32_t tpool_cap;
+  FastMod tbkt_mod[kMaxTables];
 };
 
 // address of tile T's replies (T counted from the start of the batch) when the replies are segmented by source

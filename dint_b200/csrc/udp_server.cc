@@ -31,7 +31,7 @@
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
 //                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
-//                        [--store-ebpf wb-bloom|wb|wt]
+//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf]
 //
 // --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
 // the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
@@ -41,6 +41,12 @@
 // store_wb_kern.c, store_wt_kern.c for V = wb-bloom, wb, wt), with its per-bucket cache sets in front of the table; the
 // server starts empty and --populate N serves the eBPF client's kInsert stream for N subscribers
 // (store/caladan/client_ebpf.cc:137-180).
+//
+// --tatp-ebpf (tatp): DINT_CFG_TATP_EBPF -- answer as the reference's eBPF TATP shard server (tatp/ebpf/shard_kern.c;
+// with --lock-holder-keys, lock_kern.c), with its per-bucket cache sets and bloom words in front of chained tables; the
+// server starts empty and --populate N serves the eBPF client's insert stream for N subscribers
+// (tatp/caladan/client_ebpf_shard.cc:96-339).  Every reply is one 55-byte struct message: the reference sends a
+// kCommitBck that missed its cache back as the 108-byte ext_message (shard_kern.c:1231), whose first 55 bytes these are.
 //
 // --mon-port P: the reference servers' utilisation channel (tatp/udp/server_shard.cc:213-274: a thread samples the CPU
 // time of the server's cores once a second, another answers any datagram on UDP :20231 with `struct {double ucores;
@@ -116,7 +122,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -128,11 +134,12 @@ int main(int argc, char** argv) {
   if (n_sock > 8) n_sock = 8;                         // the reference runs `server 8` (exp/run_lock_fasst.sh)
   std::string bind_addr = "0.0.0.0";
   std::vector<int> devices;
-  bool holder_keys = false;
+  bool holder_keys = false, tatp_ebpf = false;
   uint32_t store_ebpf = 0;
   for (int i = 2; i < argc; i += 2) {
     const std::string a = argv[i];
-    if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the one option without a value
+    if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the two options without a value
+    if (a == "--tatp-ebpf") { tatp_ebpf = true; i--; continue; }
     if (i + 1 >= argc) break;
     const char* v = argv[i + 1];
     if (a == "--port") port = atoi(v);
@@ -172,6 +179,7 @@ int main(int argc, char** argv) {
   dint_default_cfg(kind, &cfg);                       // kLockHashSize, table sizes, ring length of the reference
   if (holder_keys) cfg.flags |= DINT_CFG_LOCK_HOLDER_KEYS;   // dint_create refuses it for a kind other than tatp
   cfg.flags |= store_ebpf;                                   // ... and this for a kind other than store
+  if (tatp_ebpf) cfg.flags |= DINT_CFG_TATP_EBPF;            // ... and this for a kind other than tatp
   if (populate >= 0) { cfg.subs_populate = (uint32_t)populate; cfg.accts_populate = (uint32_t)populate; }   // a prefix of the reference's population
   dint_engine* eng = nullptr;
   dint_cluster* cluster = nullptr;

@@ -57,6 +57,13 @@ class Tatp:               # tatp/udp/net.h:15-52
     kSubscriber, kSecondSubscriber, kAccessInfo, kSpecialFacility, kCallForwarding = range(5)
 
 
+class TatpEbpf:           # tatp/ebpf/utils.h:40-73: the eBPF TATP shard server's packet types (the same values)
+    (READ, ACQUIRE_LOCK, ABORT, COMMIT, GRANT_READ, REJECT_READ, NOT_EXIST, GRANT_LOCK, REJECT_LOCK, ABORT_ACK,
+     COMMIT_ACK, REJECT_COMMIT, COMMIT_PRIM, COMMIT_BCK, COMMIT_LOG, COMMIT_PRIM_ACK, COMMIT_BCK_ACK, COMMIT_LOG_ACK,
+     INSERT_PRIM, INSERT_BCK, INSERT_PRIM_ACK, INSERT_BCK_ACK, DELETE_PRIM, DELETE_BCK, DELETE_LOG, DELETE_PRIM_ACK,
+     DELETE_BCK_ACK, DELETE_LOG_ACK, REJECT_LOCK_SAME_KEY) = range(29)
+
+
 class Smallbank:          # smallbank/udp/net.h:15-38
     (kAcquireShared, kAcquireExclusive, kReleaseShared, kReleaseExclusive, kCommitPrim, kCommitBck,
      kCommitLog, kGrantShared, kRejectShared, kGrantExclusive, kRejectExclusive, kReleaseSharedAck,

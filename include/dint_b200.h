@@ -123,6 +123,46 @@ typedef struct dint_cfg {
 #define DINT_CFG_STORE_EBPF_MASK (3u << 1)
 #define DINT_STORE_CACHE_ENTRY_BYTES 232         /* sizeof(struct cache_entry), store/ebpf/utils.h:58-66 */
 
+/*
+ * dint_cfg.flags bit 3, tatp only (dint_create / dint_cluster_create answer DINT_EINVAL for another kind, and
+ * dint_create for n_shards > 1: place tatp shards with txn_shards): answer as the reference's eBPF TATP shard server
+ * (tatp/ebpf/shard_kern.c with shard_user.c) instead of its UDP server (tatp/udp/server_shard.cc).  Together with
+ * DINT_CFG_LOCK_HOLDER_KEYS it is tatp/ebpf/lock_kern.c.  The eBPF server keeps a 4-slot write-back cache set with a
+ * bloom word per bucket of all five tables in XDP maps, answers hits and the lock traffic there, passes misses to a
+ * user-space chained `kvs` and installs the answer from a TC egress program.  The tier leaks into the wire, so the
+ * cache, the bloom words and the chained tables are modelled exactly:
+ *   - sizes (tatp/ebpf/utils.h:11-21): subscriber and secondary subscriber S*3/2/4 buckets, access info, special
+ *     facility AND call forwarding S*15/4/4 (the UDP server gives call forwarding S*45/8/4); 4 lock slots per bucket;
+ *   - kRead: a hit answers from the set and sets the key's bloom bit (the top 6 bits of fasthash64(key)); a miss whose
+ *     bit is clear is answered kNotExist with the request's ver; otherwise the table answers, after a dirty victim
+ *     (first invalid slot, else first clean, else slot 0) was written back; a kNotExist from the table carries the
+ *     eviction flag (0 / 1) in ver;
+ *   - kCommitPrim / kCommitBck: a hit updates the set (ver + 1, dirty) and echoes the client's ver; a miss returns the
+ *     TABLE's new version (0 when kvs_set inserted the row);
+ *   - kInsertPrim / kInsertBck without a dirty victim put the row ONLY into the cache, dirty, with ver 0: the table
+ *     sees it when it is evicted, by kvs_set(key, val, ver), which INCREMENTS the table's version when ver is 0 and
+ *     inserts the row with version 0 when the table lacks it.  Over a dirty victim the row goes into the table too;
+ *   - kDeletePrim / kDeleteBck: the first 8 value bytes of the reply are the bucket's rebuilt bloom word, one bit per
+ *     CHAIN ENTRY of fasthash64 over its whole 32-byte key array (stale keys of invalid slots included,
+ *     shard_user.c:94-104), so a later read of a key the table holds may be answered kNotExist;
+ *   - a key inserted twice is kept twice by the chained table, and lookups find the copy nearer the chain's head;
+ *   - the reference sends a kCommitBck miss back as its 108-byte ext_message (shard_kern.c:1231); the engine's reply
+ *     is that datagram's first 55 bytes, which is what a client reading a struct message sees.
+ * kReject* / kRetry replies (a set locked by another server thread) are never produced.  A type shard_user.c panics on
+ * or a table >= 5 is answered 0xFF (DINT_EPROTO), as is a request that needed a chain entry when the engine's pool of
+ * 1.5 entries per bucket was exhausted (counted in dint_tatp_cache_stats; the reference's calloc never fails); what
+ * that request changed before the failed allocation (its cache set, a write-back) stays.
+ * The server starts EMPTY: dint_populate serves the eBPF client's insert stream (tatp/caladan/client_ebpf_shard.cc:
+ * 96-339, 600 populate threads in thread order) through the tier, kInsertPrim where this engine is the row's primary
+ * (key % 3 == txn_shard_id; key % txn_shards when txn_shards > 3) and kInsertBck where it is a backup; dint_load serves
+ * its pairs as kInsertBck requests (which leave the lock words alone).  Costs 256 bytes of HBM per bucket for the sets and 384 for the chain pool (6.4 + 9.6 GB at
+ * S = 7,000,000).  Without the bit nothing is allocated and the engine answers as tatp/udp/server_shard.cc.
+ * dint_lock_state / dint_lock_holder take the reference's lock slot (dint_lock_slot); dint_kv_get / dint_kv_count
+ * answer from the chained tables, as kvs_get would.
+ */
+#define DINT_CFG_TATP_EBPF (1u << 3)
+#define DINT_TATP_CHAIN_REC_BYTES 212   /* {u64 key[4]; u32 ver[4]; u8 valid[4]; u8 val[4][40]}, tatp/ebpf/kvs.h:13-19 */
+
 typedef struct dint_engine dint_engine;
 
 /* Counters since create (or the last dint_reset_stats). */
@@ -305,6 +345,16 @@ int dint_store_cache_set(dint_engine *e, uint32_t bucket, void *out);
  * served by the backing table (the user-space path), [3] dirty victims written back, [4] slots filled (installs and
  * cached inserts). */
 int dint_store_cache_stats(dint_engine *e, uint64_t out[5]);
+/* Cache set `bucket` (fasthash64(key) % the table's bucket count) of table `table` of a tatp engine with
+ * DINT_CFG_TATP_EBPF, as the reference's struct cache_entry (232 bytes, tatp/ebpf/utils.h:103-111; lock = 0). */
+int dint_tatp_cache_set(dint_engine *e, int table, uint32_t bucket, void *out);
+/* The chain of that bucket, head first: *n = its length, and the first min(n, max) entries written to `out` as
+ * DINT_TATP_CHAIN_REC_BYTES records (stale keys of invalid slots as the table left them). */
+int dint_tatp_chain(dint_engine *e, int table, uint32_t bucket, void *out, uint32_t max, uint32_t *n);
+/* The tier's counters since create: out[0] requests answered from the cache (hits), [1] bloom negatives, [2] requests
+ * served by the user-space path, [3] dirty victims written back, [4] slots filled, [5] chain entries allocated from
+ * the pool, [6] entries reused from the bucket's freed ones, [7] entries freed, [8] allocations that failed. */
+int dint_tatp_cache_stats(dint_engine *e, uint64_t out[9]);
 int64_t dint_kv_count(dint_engine *e, int table);
 /* lock_2pl: out = {num_ex, num_sh}; lock_fasst: {lock, ver}; tatp: {lock, 0}; smallbank: {num_ex, num_sh} */
 int dint_lock_state(dint_engine *e, int table, uint32_t slot, uint32_t out[2]);
