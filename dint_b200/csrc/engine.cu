@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <algorithm>
 #include <chrono>
 #include <type_traits>
 #include <vector>
@@ -43,6 +44,8 @@ static const uint32_t kValSize[DINT_NUM_KINDS] = {0, 0, 0, 40, 40, 8};
 constexpr int kExecStoreEbpf = DINT_NUM_KINDS;
 // ... and of a tatp engine with the eBPF cache tier (DINT_CFG_TATP_EBPF)
 constexpr int kExecTatpEbpf = DINT_NUM_KINDS + 1;
+// ... and of a smallbank engine with the eBPF cache tier (DINT_CFG_SMALLBANK_EBPF)
+constexpr int kExecSmallbankEbpf = DINT_NUM_KINDS + 2;
 
 // The one place where an engine's run-time kind picks the kernel templates: calls f(std::integral_constant<int, K>{})
 // and returns what f returns.  Record-size-keyed kernels are instantiated with Wire<K>::MSG.
@@ -57,6 +60,7 @@ static int with_kind(int kind, F&& f) {
     case DINT_SMALLBANK: return f(std::integral_constant<int, K_SMALLBANK>{});
     case kExecStoreEbpf: return f(std::integral_constant<int, K_STORE_EBPF>{});
     case kExecTatpEbpf: return f(std::integral_constant<int, K_TATP_EBPF>{});
+    case kExecSmallbankEbpf: return f(std::integral_constant<int, K_SMALLBANK_EBPF>{});
   }
   return set_err(DINT_EINVAL, "bad kind");
 }
@@ -146,9 +150,11 @@ struct dint_engine {
   KvHost kv[kMaxTables];
 };
 
-// the kind whose kernels serve this engine: its public kind, or the store's / tatp's cache-tier kind
+// a smallbank engine with the eBPF cache tier (its sets live in ctx.ecache, as the store's do)
+static bool sbe_on(const dint_engine* e) { return e->kind == DINT_SMALLBANK && e->ctx.ecache; }
+// the kind whose kernels serve this engine: its public kind, or the store's / tatp's / smallbank's cache-tier kind
 static int exec_kind(const dint_engine* e) {
-  return e->ctx.tchain ? kExecTatpEbpf : e->ctx.ecache ? kExecStoreEbpf : e->kind;
+  return e->ctx.tchain ? kExecTatpEbpf : sbe_on(e) ? kExecSmallbankEbpf : e->ctx.ecache ? kExecStoreEbpf : e->kind;
 }
 
 template <typename T>
@@ -384,7 +390,7 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
       ProfScope ps(e, s, KT_LOAD);
       with_kind(exec_kind(e), [&](auto k) {
         constexpr int K = decltype(k)::value;
-        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
+        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK || K == K_SMALLBANK_EBPF) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
         return DINT_OK;
       });
     }
@@ -678,6 +684,13 @@ static int create_impl(dint_engine* e) {
     if ((rc = dalloc(e, &c.tpool, (size_t)c.tpool_cap * kTeEntBytes))) return rc;
     if ((rc = dalloc(e, &c.tpool_top, 1))) return rc;
   }
+  // the eBPF SmallBank server's cache sets (smallbank/ebpf/shard_kern.c:40-52): one 128-byte set per bucket of both
+  // tables (groups / 4: four lock slots per bucket), zeroed = every slot invalid, as the reference's cache starts
+  if (cf.flags & DINT_CFG_SMALLBANK_EBPF) {
+    for (uint32_t t = 0; t < c.n_tables; t++) c.tbkt_mod[t] = make_fastmod(e->kv[t].hash_size);
+    if ((rc = dalloc(e, &c.ecache, groups / 4 * kSbeSetBytes))) return rc;
+    if ((rc = dalloc(e, &c.ecache_stats, SBE_NSTATS))) return rc;
+  }
   {
     uint32_t fl = 25;                                  // 2^25 nibbles = 16 MB per set: L2-resident
     while (fl > 10 && (1ULL << (fl - 1)) >= groups * 2 + 2048) fl--;   // tiny group spaces need less
@@ -768,6 +781,8 @@ int dint_create(int kind, const dint_cfg* cfg, int device, dint_engine** out) {
   if ((cf.flags & DINT_CFG_STORE_EBPF_MASK) && kind != DINT_STORE) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_STORE_EBPF_* is a store option"); }
   if ((cf.flags & DINT_CFG_TATP_EBPF) && kind != DINT_TATP) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_TATP_EBPF is a tatp option"); }
   if ((cf.flags & DINT_CFG_TATP_EBPF) && cf.n_shards != 1) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_TATP_EBPF needs n_shards = 1 (place tatp shards with txn_shards)"); }
+  if ((cf.flags & DINT_CFG_SMALLBANK_EBPF) && kind != DINT_SMALLBANK) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_SMALLBANK_EBPF is a smallbank option"); }
+  if ((cf.flags & DINT_CFG_SMALLBANK_EBPF) && cf.n_shards != 1) { delete e; return set_err(DINT_EINVAL, "DINT_CFG_SMALLBANK_EBPF needs n_shards = 1 (place smallbank shards with txn_shards)"); }
   if (cf.chunk == 0) cf.chunk = 1u << 20;
   e->chunk = (cf.chunk + kTile - 1) / kTile * kTile;
   {
@@ -1017,7 +1032,8 @@ static void snapshot_regions(dint_engine* e, std::vector<std::pair<void*, size_t
     r.push_back({c.tchain, g / 4 * sizeof(uint2)});
     r.push_back({c.tpool, (size_t)c.tpool_cap * kTeEntBytes});
     r.push_back({c.tpool_top, sizeof(uint32_t)});
-  } else if (c.ecache) r.push_back({c.ecache, g * kEcSetBytes});
+  } else if (sbe_on(e)) r.push_back({c.ecache, g / 4 * kSbeSetBytes});
+  else if (c.ecache) r.push_back({c.ecache, g * kEcSetBytes});
   for (uint32_t t = 0; t < c.n_tables; t++) {
     r.push_back({c.tbl[t].entries, (size_t)(c.tbl[t].cap_mask + 1) << c.tbl[t].ent_shift});
     r.push_back({c.tbl[t].live, 16});
@@ -1067,7 +1083,7 @@ void dint_snapshot_destroy(dint_snapshot* s) {
   delete s;
 }
 
-// lock position of lock slot `slot` (= b + H j) of a table of the eBPF TATP tier: 4 b + j (kv.cuh, te_lock_pos)
+// lock position of lock slot `slot` (= b + H j) of a table of the eBPF TATP / SmallBank tier: 4 b + j (kv.cuh, te_lock_pos)
 static uint32_t te_lock_pos_host(const Ctx& c, int table, uint32_t slot) {
   const uint32_t H = c.tbkt_mod[table].d;
   return c.tbl[table].grp_base + 4 * (slot % H) + slot / H;
@@ -1084,7 +1100,7 @@ int dint_lock_state(dint_engine* e, int table, uint32_t slot, uint32_t out[2]) {
     if (table < 0 || table >= (int)c.n_tables) return DINT_EINVAL;
     if (slot % c.n_shards != c.shard_id) return DINT_EINVAL;
     g = c.tbl[table].grp_base + slot / c.n_shards;
-    if (c.tchain) {
+    if (c.tchain || sbe_on(e)) {
       if (slot >= c.tbl[table].n_groups) return DINT_EINVAL;   // 4H lock slots per table
       g = te_lock_pos_host(c, table, slot);
     }
@@ -1238,7 +1254,7 @@ int dint_load(dint_engine* e, int table, const uint64_t* keys, const void* vals,
   if (!e || table < 0 || table >= (int)e->ctx.n_tables || (n && (!keys || !vals))) return set_err(DINT_EINVAL, "bad table/arguments");
   CU(cudaSetDevice(e->device));
   if (e->ctx.tchain) return te_serve_inserts(e, table, keys, (const uint8_t*)vals, n, false);
-  if (e->ctx.ecache) return ec_serve_inserts(e, keys, (const uint8_t*)vals, n);
+  if (e->ctx.ecache && e->kind == DINT_STORE) return ec_serve_inserts(e, keys, (const uint8_t*)vals, n);
   const uint32_t vs = kValSize[e->kind];
   const uint64_t batch = 1u << 20;
   uint64_t* dk = nullptr;
@@ -1273,6 +1289,42 @@ int dint_load(dint_engine* e, int table, const uint64_t* keys, const void* vals,
   return rc;
 }
 
+// The eBPF SmallBank client's warm-up (smallbank/caladan/client_ebpf_shard.cc:88-169, 1526-1545): kWarmupRead of
+// (saving, a) then (checking, a) for every account a < accts_populate this shard replicates (all of them with
+// txn_shards <= 3; a % G in {I - 2, I - 1, I} with G = txn_shards > 3), ascending -- the 600 warm-up threads' slices
+// taken in thread order.  Generated on the device (k_sbe_warmup) and served in batches through dint_submit_device.
+static int sbe_warmup(dint_engine* e) {
+  const uint64_t A = e->cfg.accts_populate;
+  const uint32_t G = e->cfg.txn_shards, me = e->cfg.txn_shard_id;
+  uint32_t per = 1, blk = 1;
+  uint32_t r[3] = {0, 0, 0};
+  uint64_t accts = A;
+  if (G > 3) {
+    per = 3; blk = G;
+    for (uint32_t k = 0; k < 3; k++) r[k] = (me + G - 2 + k) % G;
+    std::sort(r, r + 3);
+    accts = A / G * 3;
+    for (uint32_t k = 0; k < 3; k++) accts += r[k] < A % G;
+  }
+  const uint64_t n = 2 * accts, batch = 1u << 22;
+  if (n == 0) return DINT_OK;
+  using W = Wire<K_SMALLBANK_EBPF>;
+  uint8_t *d_req = nullptr, *d_resp = nullptr;
+  CU(cudaMalloc(&d_req, batch * W::MSG));
+  cudaError_t ce = cudaMalloc(&d_resp, batch * W::MSG);
+  if (ce != cudaSuccess) { cudaFree(d_req); return set_err(DINT_ENOMEM, "cudaMalloc", ce); }
+  int rc = DINT_OK;
+  for (uint64_t off = 0; off < n && rc == DINT_OK; off += batch) {
+    const uint32_t m = (uint32_t)(n - off < batch ? n - off : batch);
+    k_sbe_warmup<<<(m + 255) / 256, 256>>>(d_req, off, m, per, blk, make_uint4(r[0], r[1], r[2], 0));
+    rc = dint_submit_device(e, d_req, m, d_resp, nullptr);
+  }
+  if (rc == DINT_OK && cudaDeviceSynchronize() != cudaSuccess) rc = set_err(DINT_EIO, "warm-up", cudaGetLastError());
+  cudaFree(d_req);
+  cudaFree(d_resp);
+  return rc;
+}
+
 int dint_populate(dint_engine* e) {
   if (!e) return DINT_EINVAL;
   if (e->ctx.n_tables == 0) return DINT_OK;       // lock / log servers start from zeroed arrays
@@ -1280,6 +1332,12 @@ int dint_populate(dint_engine* e) {
     return tatp_ebpf_populate(e->cfg, [&](int table, const uint64_t* k, const void* v, uint64_t n) {
       return te_serve_inserts(e, table, k, (const uint8_t*)v, n, true);
     });
+  }
+  if (sbe_on(e)) {                                // the eBPF SmallBank server: kvs_insert of every account, then
+    int rc = kv_populate(e->kind, e->cfg, [&](int table, const uint64_t* k, const void* v, uint64_t n) {
+      return dint_load(e, table, k, v, n);
+    });
+    return rc ? rc : sbe_warmup(e);               // ... its client's warm-up through the tier
   }
   if (e->ctx.ecache) {                            // the eBPF store starts empty and is filled over the wire
     return store_ebpf_populate(e->cfg, [&](int, const uint64_t* k, const void* v, uint64_t n) {
@@ -1383,8 +1441,36 @@ int dint_tatp_cache_stats(dint_engine* e, uint64_t out[9]) {
   return DINT_OK;
 }
 
+int dint_smallbank_cache_set(dint_engine* e, int table, uint32_t bucket, void* out) {
+  if (!e || !out || !sbe_on(e)) return set_err(DINT_EINVAL, "not a smallbank engine with the eBPF cache tier");
+  const Ctx& c = e->ctx;
+  if (table < 0 || table >= (int)c.n_tables || bucket >= c.tbkt_mod[table].d) return set_err(DINT_EINVAL, "bad table / bucket");
+  CU(cudaSetDevice(e->device));
+  CU(cudaDeviceSynchronize());
+  uint8_t s[kSbeSetBytes];
+  CU(cudaMemcpy(s, c.ecache + (size_t)(c.tbl[table].grp_base / 4 + bucket) * kSbeSetBytes, sizeof s, cudaMemcpyDeviceToHost));
+  uint8_t* o = (uint8_t*)out;                      // struct cache_entry, smallbank/ebpf/utils.h:82-89
+  memset(o, 0, DINT_SMALLBANK_CACHE_ENTRY_BYTES);
+  memcpy(o, s, 32);                                // key[4]
+  memcpy(o + 32, s + 64, 32);                      // val[4][8]
+  memcpy(o + 64, s + 32, 16);                      // ver[4]
+  for (int i = 0; i < 4; i++) {
+    o[80 + i] = (s[48] >> i) & 1;                  // valid[4]
+    o[84 + i] = (s[49] >> i) & 1;                  // dirty[4]; lock (+88) = 0
+  }
+  return DINT_OK;
+}
+
+int dint_smallbank_cache_stats(dint_engine* e, uint64_t out[4]) {
+  if (!e || !out || !sbe_on(e)) return set_err(DINT_EINVAL, "not a smallbank engine with the eBPF cache tier");
+  CU(cudaSetDevice(e->device));
+  CU(cudaDeviceSynchronize());
+  CU(cudaMemcpy(out, e->ctx.ecache_stats, SBE_NSTATS * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  return DINT_OK;
+}
+
 int dint_store_cache_set(dint_engine* e, uint32_t bucket, void* out) {
-  if (!e || !out || !e->ctx.ecache || e->ctx.tchain) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
+  if (!e || !out || !e->ctx.ecache || e->kind != DINT_STORE) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
   const Ctx& c = e->ctx;
   if (bucket % c.n_shards != c.shard_id || bucket / c.n_shards >= e->total_groups) return set_err(DINT_EINVAL, "bucket of another shard");
   CU(cudaSetDevice(e->device));
@@ -1396,7 +1482,7 @@ int dint_store_cache_set(dint_engine* e, uint32_t bucket, void* out) {
 }
 
 int dint_store_cache_stats(dint_engine* e, uint64_t out[5]) {
-  if (!e || !out || !e->ctx.ecache || e->ctx.tchain) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
+  if (!e || !out || !e->ctx.ecache || e->kind != DINT_STORE) return set_err(DINT_EINVAL, "not a store engine with the eBPF cache tier");
   CU(cudaSetDevice(e->device));
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out, e->ctx.ecache_stats, EC_NSTATS * sizeof(uint64_t), cudaMemcpyDeviceToHost));
@@ -1796,6 +1882,7 @@ int dint_cluster_create(int kind, const dint_cfg* cfg, int n_gpus, const int* de
   if (cfg && (cfg->flags & DINT_CFG_LOCK_HOLDER_KEYS) && kind != DINT_TATP) return set_err(DINT_EINVAL, "DINT_CFG_LOCK_HOLDER_KEYS is a tatp option");
   if (cfg && (cfg->flags & DINT_CFG_STORE_EBPF_MASK) && kind != DINT_STORE) return set_err(DINT_EINVAL, "DINT_CFG_STORE_EBPF_* is a store option");
   if (cfg && (cfg->flags & DINT_CFG_TATP_EBPF) && kind != DINT_TATP) return set_err(DINT_EINVAL, "DINT_CFG_TATP_EBPF is a tatp option");
+  if (cfg && (cfg->flags & DINT_CFG_SMALLBANK_EBPF) && kind != DINT_SMALLBANK) return set_err(DINT_EINVAL, "DINT_CFG_SMALLBANK_EBPF is a smallbank option");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return set_err(DINT_ENODEV, "no CUDA device: dint_b200 has no CPU fallback"); }
   dint_cluster* cl = new dint_cluster();

@@ -38,9 +38,11 @@ namespace dint {
 
 enum Kind { K_LOCK2PL = 0, K_FASST = 1, K_LOG = 2, K_STORE = 3, K_TATP = 4, K_SMALLBANK = 5,
             K_STORE_EBPF = 6,     // internal: a store engine created with a DINT_CFG_STORE_EBPF_* variant (kv.cuh)
-            K_TATP_EBPF = 7 };    // internal: a tatp engine created with DINT_CFG_TATP_EBPF (kv.cuh)
+            K_TATP_EBPF = 7,      // internal: a tatp engine created with DINT_CFG_TATP_EBPF (kv.cuh)
+            K_SMALLBANK_EBPF = 8 };   // internal: a smallbank engine created with DINT_CFG_SMALLBANK_EBPF (kv.cuh)
 // the kinds whose requests append to a commit log (K1 counts the appends per tile, K1b turns them into ring ordinals)
-template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK || KIND == K_TATP_EBPF;
+template <int KIND> constexpr bool kHasLog = KIND == K_LOG || KIND == K_TATP || KIND == K_SMALLBANK || KIND == K_TATP_EBPF ||
+                                            KIND == K_SMALLBANK_EBPF;
 
 constexpr int kTile = 128;       // wire records per tile = threads per CTA in K1/K2 (16 CTAs, i.e. 16 independent
                                  // latency chains, per SM)
@@ -78,6 +80,7 @@ template <> struct Wire<K_TATP_EBPF> : Wire<K_TATP> {};     // tatp/ebpf/utils.h
 template <> struct Wire<K_SMALLBANK> { // smallbank/udp/net.h:43-52 {u8 ord; u8 type; u8 table; u64 key; u8 val[8]; u32 ver}
   static constexpr int MSG = 23, TYPE = 1, TABLE = 2, KEY = 3, VAL = 11, VER = 19, VALSZ = 8, LOGENT = 32;
 };
+template <> struct Wire<K_SMALLBANK_EBPF> : Wire<K_SMALLBANK> {};   // smallbank/ebpf/utils.h:60-67 (same shape)
 
 // ---- KV table: open addressing, one 64-byte (val 40) or 32-byte (val 8) entry per key -------------
 // entry = { u64 key; u32 ver; u32 meta; u8 val[VALSZ]; pad } -- a GET that hits on its first probe
@@ -167,6 +170,8 @@ struct Ctx {
   // `ecache_stats` the tier's counters (EC_NSTATS_TATP); the chained tables are a {head, free list} pair per bucket
   // (entry index + 1, 0 = none) over one pool of 256-byte chain entries with a bump allocator; tbkt_mod = the bucket
   // count of each table.  Null / 0 without the option.
+  // smallbank with the eBPF cache tier (DINT_CFG_SMALLBANK_EBPF): `ecache` holds one 128-byte cache set per bucket of
+  // both tables, `ecache_stats` the tier's counters (SBE_NSTATS) and tbkt_mod the bucket counts; tchain stays null.
   uint2* tchain;
   uint8_t* tpool;
   uint32_t* tpool_top;

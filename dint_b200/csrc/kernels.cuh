@@ -141,7 +141,7 @@ DINT_D uint32_t route_owner_of(const Ctx& c, const uint8_t* rec) {
   uint32_t gglobal = 0;
   if constexpr (KIND == K_LOCK2PL || KIND == K_FASST) gglobal = fast_mod(fasthash64_u32(ld_u32_unaligned(rec + W::KEY)), c.slot_mod);
   else if constexpr (KIND == K_STORE || KIND == K_STORE_EBPF) gglobal = fast_mod(fasthash64_u64(ld_u64_unaligned(rec + W::KEY)), c.tbl[0].lock_mod);
-  else if constexpr (KIND == K_TATP || KIND == K_TATP_EBPF || KIND == K_SMALLBANK) gglobal = fast_mod(fasthash64_u64(ld_u64_unaligned(rec + W::KEY)), c.tbl[rec[W::TABLE]].lock_mod);
+  else if constexpr (KIND == K_TATP || KIND == K_TATP_EBPF || KIND == K_SMALLBANK || KIND == K_SMALLBANK_EBPF) gglobal = fast_mod(fasthash64_u64(ld_u64_unaligned(rec + W::KEY)), c.tbl[rec[W::TABLE]].lock_mod);
   else return c.shard_id;
   return gglobal - (uint32_t)fast_div(gglobal, c.shard_div) * c.n_shards;
 }

@@ -97,6 +97,20 @@ DINT_D bool kv_set_from(const KvTable& t, uint64_t key, uint64_t h, uint4 (&v)[E
   *((uint32_t*)(e + 8)) = v[0].z + 1;
   return true;
 }
+// kvs_set of the eBPF servers (smallbank/ebpf/kvs.h:55-74): overwrite val; ver = `ver` when non-zero, else ver + 1.
+// `nv` = the new version.  Probes afresh (earlier calls of the same request may have written).
+template <int VALSZ>
+DINT_D bool kv_set_ver(const KvTable& t, uint64_t key, uint64_t h, const uint32_t (&w)[Ent<VALSZ>::NW], uint32_t ver,
+                       uint32_t& nv) {
+  uint4 v[Ent<VALSZ>::NV];
+  kv_load_entry<VALSZ>(t.entries + (kv_home(t, h) << t.ent_shift), v);
+  uint8_t* e = kv_find<VALSZ>(t, key, h, v);
+  if (!e) return false;
+  kv_write_val<VALSZ>(e, w);
+  nv = ver != 0 ? ver : v[0].z + 1;
+  *((uint32_t*)(e + 8)) = nv;
+  return true;
+}
 
 // kvs_insert (kvs.h:77-104): take the first free entry on the probe path, ver = 0.  Like the
 // reference it does not look for an existing copy of the key.
@@ -910,24 +924,27 @@ template <> DINT_D Pre<K_SMALLBANK> prefetch_coop<K_SMALLBANK>(const Ctx& c, con
   kv_prefetch_home_coop<8>(need ? kv_home_ptr<8>(c, rec[W::TABLE], ki.h) : nullptr, need, p.v);
   return p;
 }
+// kCommitLog (smallbank/udp/server_shard.cc:175-186); the eBPF server's XDP path (smallbank/ebpf/shard_kern.c:566-583)
+// writes the same entry, whatever the table byte
+DINT_D void smallbank_log_append(const Ctx& c, uint8_t* rec, uint8_t table, unsigned long long ord, bool keep) {
+  using W = Wire<K_SMALLBANK>;
+  if (keep) {                              // log_entry {table@0 key@8 val@16 ver@24}
+    uint8_t* e = c.ring + (size_t)(ord % c.ring_n) * W::LOGENT;
+    uint32_t w[5];
+    ld_words_unaligned<5>(rec + W::KEY, w);
+    e[0] = table;
+    *((uint2*)(e + 8)) = make_uint2(w[0], w[1]);
+    *((uint2*)(e + 16)) = make_uint2(w[2], w[3]);
+    *((uint32_t*)(e + 24)) = w[4];
+  }
+  rec[W::TYPE] = 15;
+}
 template <>
 DINT_D void apply_one<K_SMALLBANK>(const Ctx& c, uint8_t* rec, const KeyInfo& ki, const Pre<K_SMALLBANK>& pf,
                                    unsigned long long ord, bool keep) {
   using W = Wire<K_SMALLBANK>;
   const uint8_t type = rec[W::TYPE], table = rec[W::TABLE];
-  if (type == 6) {                         // kCommitLog :175-186; log_entry {table@0 key@8 val@16 ver@24}
-    if (keep) {
-      uint8_t* e = c.ring + (size_t)(ord % c.ring_n) * W::LOGENT;
-      uint32_t w[5];
-      ld_words_unaligned<5>(rec + W::KEY, w);
-      e[0] = table;
-      *((uint2*)(e + 8)) = make_uint2(w[0], w[1]);
-      *((uint2*)(e + 16)) = make_uint2(w[2], w[3]);
-      *((uint32_t*)(e + 24)) = w[4];
-    }
-    rec[W::TYPE] = 15;
-    return;
-  }
+  if (type == 6) { smallbank_log_append(c, rec, table, ord, keep); return; }
   const KvTable& t = c.tbl[table];
   const uint64_t key = ki.key, h = ki.h;
   const uint32_t g = ki.grp;
@@ -948,6 +965,155 @@ DINT_D void apply_one<K_SMALLBANK>(const Ctx& c, uint8_t* rec, const KeyInfo& ki
     rec[W::TYPE] = (type == 4) ? 13 : 14;
   }
   if (!ok) mark_invalid<K_SMALLBANK>(c, rec);   // smallbank/udp/kvs.h:67,86 panic
+}
+
+// ============================ smallbank, eBPF cache tier (DINT_CFG_SMALLBANK_EBPF) ==================
+// The reference's eBPF SmallBank shard server (smallbank/ebpf/shard_kern.c): an XDP program keeps the lock units and a
+// 4-slot write-back cache set per bucket of both tables, answers lock traffic and cache hits itself, passes misses to
+// user space (shard_user.c:139-189, over smallbank/ebpf/kvs.h) and installs the table's answer from a TC egress program
+// (shard_kern.c:671-741).  apply_one<K_SMALLBANK_EBPF> is that whole path for one request.  There is no bloom word, no
+// insert and no delete, so the table side is the open-addressing table of K_SMALLBANK: population inserts a key once,
+// and kvs_get / kvs_set find that one copy whatever the chain layout is.
+// Cache set, 128 bytes: tag block {u64 key[4]; u32 ver[4]; u32 valid_mask | dirty_mask << 8; pad} at +0 (one 64-byte
+// fetch decides hit / victim), u64 val[4] at +64.  Conflict group = (table, bucket), numbered and laid out as
+// K_TATP_EBPF's (te_lock_pos): the {num_ex, num_sh} counters stay one per lock slot h % 4H, at grp_base + 4 b + j.
+enum : uint32_t { SBE_HIT = 0, SBE_TABLE = 1, SBE_WRITEBACK = 2, SBE_INSTALL = 3, SBE_NSTATS = 4 };
+constexpr uint32_t kSbeSetBytes = 128;
+
+template <> DINT_D TypeInfo type_info<K_SMALLBANK_EBPF>(const uint8_t* rec) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  if (rec[W::TYPE] == 6) return TypeInfo{0, false, true};          // kCommitLog: the table byte is never checked
+  if (rec[W::TABLE] >= 2) return TypeInfo{0, true, false};         // XDP passes it up unextended: shard_user.c:142 panics
+  switch (rec[W::TYPE]) {
+    case 0: case 1: return TypeInfo{C_WL | C_WA, false, false};    // kAcquire*: the counters, then the set (a miss installs)
+    case 2: case 3: return TypeInfo{C_WL, false, false};           // kRelease*
+    case 4: case 5: case 17: return TypeInfo{C_WA, false, false};  // kCommitPrim / kCommitBck / kWarmupRead
+    default: return TypeInfo{0, true, false};                      // shard_user.c:142,188 panic
+  }
+}
+template <> DINT_D KeyInfo key_info<K_SMALLBANK_EBPF>(const Ctx& c, const uint8_t* rec) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  KeyInfo k;
+  k.key = ld_u64_unaligned(rec + W::KEY);
+  k.h = fasthash64_u64(k.key);
+  k.grp = te_lock_pos(c, rec[W::TABLE], k.h) >> 2;     // one engine owns the whole key space (n_shards = 1)
+  return k;
+}
+template <> struct Pre<K_SMALLBANK_EBPF> { uint4 t[4]; uint2 s; };   // the set's tag block; the lock unit's counters
+DINT_D uint8_t* sbe_set(const Ctx& c, uint32_t g) { return c.ecache + (size_t)g * kSbeSetBytes; }
+template <>
+DINT_D Pre<K_SMALLBANK_EBPF> prefetch<K_SMALLBANK_EBPF>(const Ctx& c, const uint8_t* rec, const KeyInfo& ki, const TypeInfo&) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  Pre<K_SMALLBANK_EBPF> p;
+  const uint8_t type = rec[W::TYPE];
+  if (type <= 3) p.s = __ldcg(&c.cnt2[te_lock_pos(c, rec[W::TABLE], ki.h)]);
+  if (type != 2 && type != 3) kv_load_entry<40>(sbe_set(c, ki.grp), p.t);
+  return p;
+}
+template <>
+DINT_D Pre<K_SMALLBANK_EBPF> prefetch_coop<K_SMALLBANK_EBPF>(const Ctx& c, const uint8_t* rec, const KeyInfo& ki,
+                                                             const TypeInfo&, bool active) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  Pre<K_SMALLBANK_EBPF> p;
+  const uint8_t type = active ? rec[W::TYPE] : 2;
+  if (active && type <= 3) p.s = __ldcg(&c.cnt2[te_lock_pos(c, rec[W::TABLE], ki.h)]);
+  const bool need = active && type != 2 && type != 3;
+  kv_prefetch_home_coop<40>(need ? sbe_set(c, ki.grp) : nullptr, need, p.t);
+  return p;
+}
+
+template <>
+DINT_D void apply_one<K_SMALLBANK_EBPF>(const Ctx& c, uint8_t* rec, const KeyInfo& ki, const Pre<K_SMALLBANK_EBPF>& pf,
+                                        unsigned long long ord, bool keep) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  const uint8_t type = rec[W::TYPE], table = rec[W::TABLE];
+  if (type == 6) { smallbank_log_append(c, rec, table, ord, keep); return; }   // shard_kern.c:566-583
+  if (type <= 3) {                                    // the lock unit (:96-392): a refusal changes nothing
+    uint2 s = pf.s;                                   // x = num_ex, y = num_sh
+    // struct lock_unit's counters are ints tested with > 0 (:138, :255): a count that a stray release took below zero
+    // refuses nothing, where the UDP server's unsigned == 0 test refuses
+    if (type == 0) {
+      if ((int32_t)s.x > 0) { rec[W::TYPE] = 8; return; }   // kRejectShared
+      s.y++;
+    } else if (type == 1) {
+      if ((int32_t)s.x > 0 || (int32_t)s.y > 0) { rec[W::TYPE] = 10; return; }   // kRejectExclusive
+      s.x++;
+    } else if (type == 2) s.y--;                      // no floor, as the UDP server
+    else s.x--;
+    c.cnt2[te_lock_pos(c, table, ki.h)] = s;          // a grant counts BEFORE the cache is looked at
+    if (type >= 2) { rec[W::TYPE] = type == 2 ? 11 : 12; return; }
+  }
+  const KvTable& t = c.tbl[table];
+  const uint64_t key = ki.key;
+  const bool commit = type == 4 || type == 5;
+  uint8_t* set = sbe_set(c, ki.grp);
+  uint32_t tw[13];                                    // tag block words: key[4] (0..7), ver[4] (8..11), masks (12)
+#pragma unroll
+  for (int k = 0; k < 3; k++) { tw[4 * k] = pf.t[k].x; tw[4 * k + 1] = pf.t[k].y; tw[4 * k + 2] = pf.t[k].z; tw[4 * k + 3] = pf.t[k].w; }
+  tw[12] = pf.t[3].x;
+  const uint32_t valid = tw[12] & 15u, dirty = (tw[12] >> 8) & 15u;
+  int hit = -1;
+#pragma unroll
+  for (int i = 3; i >= 0; i--)
+    if (((valid >> i) & 1u) && tw[2 * i] == (uint32_t)key && tw[2 * i + 1] == (uint32_t)(key >> 32)) hit = i;
+  uint32_t rw[2];                                     // the request's value
+  ld_words_unaligned<2>(rec + W::VAL, rw);
+  const uint8_t ack = type == 0 ? 7 : type == 1 ? 9 : type == 4 ? 13 : type == 5 ? 14 : 18;
+  uint32_t* tag = (uint32_t*)set;
+  if (hit >= 0) {
+    ec_count(c, SBE_HIT);
+    uint2* vp = (uint2*)(set + 64) + hit;
+    if (commit) {                                     // :424-435 / :510-521: the reply echoes the client's ver
+      *vp = make_uint2(rw[0], rw[1]);
+      tag[8 + hit] = tw[8 + hit] + 1;
+      if (!((dirty >> hit) & 1u)) tag[12] = tw[12] | (0x100u << hit);
+      rec[W::TYPE] = ack;
+    } else {                                          // :159-167, :276-284, :615-623: a warm-up hit is kGrantShared
+      const uint2 v = __ldcg(vp);
+      const uint32_t w[2] = {v.x, v.y};
+      st_words_unaligned<2>(rec + W::VAL, w);
+      st_u32_unaligned(rec + W::VER, tw[8 + hit]);
+      rec[W::TYPE] = type == 1 ? 9 : 7;
+    }
+    return;
+  }
+  // a miss: XDP picks the victim (first invalid, else first clean, else 0: :189-198) and passes the request up
+  ec_count(c, SBE_TABLE);
+  int vic = 0;
+  {
+    const uint32_t inv = ~valid & 15u, cln = ~dirty & 15u;
+    if (inv) vic = __ffs(inv) - 1;
+    else if (cln) vic = __ffs(cln) - 1;
+  }
+  if (((valid & dirty) >> vic) & 1u) {                // shard_user.c:145,154,163,172,180: kvs_set(key2, val2, ver2)
+    const uint2 ov = __ldcg((const uint2*)(set + 64) + vic);
+    const uint32_t ow[2] = {ov.x, ov.y};
+    const uint64_t okey = ((uint64_t)tw[2 * vic + 1] << 32) | tw[2 * vic];
+    uint32_t ignored;                                 // a cached key came from the table: it is there
+    (void)kv_set_ver<8>(t, okey, fasthash64_u64(okey), ow, tw[8 + vic], ignored);
+    ec_count(c, SBE_WRITEBACK);
+  }
+  uint32_t w[2] = {rw[0], rw[1]}, ver = 0;
+  bool found;
+  if (commit) {                                       // :165,173: kvs_set(key, val, 0) -> the table's new version
+    found = kv_set_ver<8>(t, key, ki.h, w, 0, ver);
+  } else {                                            // :147,156,182: kvs_get
+    uint4 v[2];
+    kv_prefetch_home<8>(c, table, ki.h, v);
+    found = kv_find<8>(t, key, ki.h, v) != nullptr;
+    w[0] = v[1].x; w[1] = v[1].y; ver = v[0].z;
+    if (found) st_words_unaligned<2>(rec + W::VAL, w);
+  }
+  // A key the table lacks: the reference's kvs_get / kvs_set panic and the server stops.  Answered 0xFF; the counter
+  // increment and the write-back above stay, and nothing is installed.
+  if (!found) { mark_invalid<K_SMALLBANK_EBPF>(c, rec); return; }
+  st_u32_unaligned(rec + W::VER, ver);
+  rec[W::TYPE] = ack;
+  *(uint2*)(set + 8 * vic) = make_uint2((uint32_t)key, (uint32_t)(key >> 32));   // TC install (:714-720), clean
+  tag[8 + vic] = ver;
+  *((uint2*)(set + 64) + vic) = make_uint2(w[0], w[1]);
+  tag[12] = (valid | (1u << vic)) | ((dirty & ~(1u << vic)) << 8);
+  ec_count(c, SBE_INSTALL);
 }
 
 // ---- bulk load (dint_load / dint_populate) and single-key inspection ------------------------------
@@ -991,6 +1157,27 @@ __global__ void __launch_bounds__(256) k_tchain_count(const Ctx c, uint32_t tabl
     if (__ldcg((const uint32_t*)(p + 56)) == table) cnt += __popc(__ldcg((const uint32_t*)(p + 48)) & 15u);
   }
   if (cnt) atomicAdd(out, (unsigned long long)cnt);
+}
+
+// The eBPF SmallBank client's warm-up stream (smallbank/caladan/client_ebpf_shard.cc:88-169) as one shard sees it:
+// record j (from `first`) is kWarmupRead of table j % 2 for the (j / 2)-th account the shard replicates, ascending --
+// account (i / per) * blk + res[i % per]: every account (per = blk = 1, res = {0}), or with G = txn_shards > 3 the
+// accounts whose a % G is one of the three residues res (per = 3, blk = G).
+__global__ void __launch_bounds__(256) k_sbe_warmup(uint8_t* out, uint64_t first, uint32_t n, uint32_t per, uint32_t blk, uint4 res) {
+  using W = Wire<K_SMALLBANK_EBPF>;
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint64_t i = (first + j) >> 1;
+  const uint32_t r = (uint32_t)(i % per);
+  const uint64_t a = i / per * blk + (r == 0 ? res.x : r == 1 ? res.y : res.z);
+  uint8_t* p = out + (size_t)j * W::MSG;
+  p[0] = 0;
+  p[W::TYPE] = 17;
+  p[W::TABLE] = (uint8_t)((first + j) & 1);
+#pragma unroll
+  for (int k = 0; k < 8; k++) p[W::KEY + k] = (uint8_t)(a >> (8 * k));
+#pragma unroll
+  for (int k = W::VAL; k < W::MSG; k++) p[k] = 0;
 }
 
 template <int VALSZ>

@@ -31,7 +31,7 @@
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
 //                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
-//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf]
+//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf]
 //
 // --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
 // the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
@@ -47,6 +47,11 @@
 // server starts empty and --populate N serves the eBPF client's insert stream for N subscribers
 // (tatp/caladan/client_ebpf_shard.cc:96-339).  Every reply is one 55-byte struct message: the reference sends a
 // kCommitBck that missed its cache back as the 108-byte ext_message (shard_kern.c:1231), whose first 55 bytes these are.
+//
+// --smallbank-ebpf (smallbank): DINT_CFG_SMALLBANK_EBPF -- answer as the reference's eBPF SmallBank shard server
+// (smallbank/ebpf/shard_kern.c), with its per-bucket write-back cache sets in front of the account tables; --populate N
+// inserts N accounts and then serves the eBPF client's warm-up stream for them (smallbank/caladan/
+// client_ebpf_shard.cc:88-169), so the cache starts as the reference's clients leave it.
 //
 // --mon-port P: the reference servers' utilisation channel (tatp/udp/server_shard.cc:213-274: a thread samples the CPU
 // time of the server's cores once a second, another answers any datagram on UDP :20231 with `struct {double ucores;
@@ -122,7 +127,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -134,12 +139,13 @@ int main(int argc, char** argv) {
   if (n_sock > 8) n_sock = 8;                         // the reference runs `server 8` (exp/run_lock_fasst.sh)
   std::string bind_addr = "0.0.0.0";
   std::vector<int> devices;
-  bool holder_keys = false, tatp_ebpf = false;
+  bool holder_keys = false, tatp_ebpf = false, smallbank_ebpf = false;
   uint32_t store_ebpf = 0;
   for (int i = 2; i < argc; i += 2) {
     const std::string a = argv[i];
-    if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the two options without a value
+    if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the three options without a value
     if (a == "--tatp-ebpf") { tatp_ebpf = true; i--; continue; }
+    if (a == "--smallbank-ebpf") { smallbank_ebpf = true; i--; continue; }
     if (i + 1 >= argc) break;
     const char* v = argv[i + 1];
     if (a == "--port") port = atoi(v);
@@ -180,6 +186,7 @@ int main(int argc, char** argv) {
   if (holder_keys) cfg.flags |= DINT_CFG_LOCK_HOLDER_KEYS;   // dint_create refuses it for a kind other than tatp
   cfg.flags |= store_ebpf;                                   // ... and this for a kind other than store
   if (tatp_ebpf) cfg.flags |= DINT_CFG_TATP_EBPF;            // ... and this for a kind other than tatp
+  if (smallbank_ebpf) cfg.flags |= DINT_CFG_SMALLBANK_EBPF;  // ... and this for a kind other than smallbank
   if (populate >= 0) { cfg.subs_populate = (uint32_t)populate; cfg.accts_populate = (uint32_t)populate; }   // a prefix of the reference's population
   dint_engine* eng = nullptr;
   dint_cluster* cluster = nullptr;

@@ -28,6 +28,11 @@ STORE_CACHE_STATS = ("hits", "bloom_negatives", "table", "write_backs", "install
 DINT_CFG_TATP_EBPF = 1 << 3
 TATP_CHAIN_REC = np.dtype([("key", "<u8", (4,)), ("ver", "<u4", (4,)), ("valid", "u1", (4,)), ("val", "u1", (4, 40))])
 TATP_CACHE_STATS = STORE_CACHE_STATS + ("allocated", "reused", "freed", "failed")
+# dint_cfg.flags bit 4 (smallbank): answer as the reference's eBPF SmallBank shard server (smallbank/ebpf/shard_kern.c):
+# a write-back cache set per bucket of both tables in front of them, warmed by dint_populate as its client warms it
+DINT_CFG_SMALLBANK_EBPF = 1 << 4
+SMALLBANK_CACHE_ENTRY_BYTES = 96   # struct cache_entry, smallbank/ebpf/utils.h:82-89
+SMALLBANK_CACHE_STATS = ("hits", "table", "write_backs", "installs")
 
 
 class DintCfg(C.Structure):
@@ -71,7 +76,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -151,6 +156,8 @@ def lib():
     L.dint_tatp_cache_set.restype = i32; L.dint_tatp_cache_set.argtypes = [vp, i32, u32, vp]
     L.dint_tatp_chain.restype = i32; L.dint_tatp_chain.argtypes = [vp, i32, u32, vp, u32, C.POINTER(u32)]
     L.dint_tatp_cache_stats.restype = i32; L.dint_tatp_cache_stats.argtypes = [vp, C.POINTER(u64)]
+    L.dint_smallbank_cache_set.restype = i32; L.dint_smallbank_cache_set.argtypes = [vp, i32, u32, vp]
+    L.dint_smallbank_cache_stats.restype = i32; L.dint_smallbank_cache_stats.argtypes = [vp, C.POINTER(u64)]
     L.dint_kv_count.restype = C.c_int64; L.dint_kv_count.argtypes = [vp, i32]
     L.dint_lock_state.restype = i32; L.dint_lock_state.argtypes = [vp, i32, u32, C.POINTER(u32)]
     L.dint_lock_holder.restype = i32; L.dint_lock_holder.argtypes = [vp, i32, u32, C.POINTER(u64)]
@@ -180,7 +187,7 @@ class DintError(RuntimeError):
 def default_cfg(kind, **over):
     """dint_default_cfg() with fields overridden by name; lock_holder_keys=True sets DINT_CFG_LOCK_HOLDER_KEYS;
     store_ebpf="wb_bloom" | "wb" | "wt" (or None) sets the DINT_CFG_STORE_EBPF_* variant; tatp_ebpf=True sets
-    DINT_CFG_TATP_EBPF."""
+    DINT_CFG_TATP_EBPF; smallbank_ebpf=True sets DINT_CFG_SMALLBANK_EBPF."""
     cfg = DintCfg()
     lib().dint_default_cfg(kind, C.byref(cfg))
     for k, v in over.items():
@@ -193,6 +200,9 @@ def default_cfg(kind, **over):
         elif k == "tatp_ebpf":
             if v:
                 cfg.flags |= DINT_CFG_TATP_EBPF
+        elif k == "smallbank_ebpf":
+            if v:
+                cfg.flags |= DINT_CFG_SMALLBANK_EBPF
         elif k == "store_ebpf":
             if v is not None:
                 if v not in STORE_EBPF_VARIANTS:
@@ -465,6 +475,22 @@ class Engine:
         if rc != 0:
             raise DintError(rc, "dint_tatp_cache_stats")
         return {k: int(out[i]) for i, k in enumerate(TATP_CACHE_STATS)}
+
+    def smallbank_cache_set(self, table, bucket):
+        """smallbank with smallbank_ebpf: cache set `bucket` of `table` as the reference's struct cache_entry (96 uint8)."""
+        out = np.zeros(SMALLBANK_CACHE_ENTRY_BYTES, dtype=np.uint8)
+        rc = lib().dint_smallbank_cache_set(self.h, table, bucket, out.ctypes.data)
+        if rc != 0:
+            raise DintError(rc, "dint_smallbank_cache_set")
+        return out
+
+    def smallbank_cache_stats(self):
+        """smallbank with smallbank_ebpf: the tier's counters since create, keyed by SMALLBANK_CACHE_STATS."""
+        out = (C.c_uint64 * 4)()
+        rc = lib().dint_smallbank_cache_stats(self.h, out)
+        if rc != 0:
+            raise DintError(rc, "dint_smallbank_cache_stats")
+        return {k: int(out[i]) for i, k in enumerate(SMALLBANK_CACHE_STATS)}
 
     def lock_slot(self, table, key):
         return lib().dint_lock_slot(self.h, table, key)

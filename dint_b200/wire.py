@@ -72,6 +72,13 @@ class Smallbank:          # smallbank/udp/net.h:15-38
     kSaving, kChecking = 0, 1
 
 
+class SmallbankEbpf:      # smallbank/ebpf/utils.h:31-50: the eBPF SmallBank shard server's packet types (the same values)
+    (ACQUIRE_SHARED, ACQUIRE_EXCLUSIVE, RELEASE_SHARED, RELEASE_EXCLUSIVE, COMMIT_PRIM, COMMIT_BCK, COMMIT_LOG,
+     GRANT_SHARED, REJECT_SHARED, GRANT_EXCLUSIVE, REJECT_EXCLUSIVE, RELEASE_SHARED_ACK, RELEASE_EXCLUSIVE_ACK,
+     COMMIT_PRIM_ACK, COMMIT_BCK_ACK, COMMIT_LOG_ACK, RETRY, WARMUP_READ, WARMUP_READ_ACK) = range(19)
+    SAVING, CHECKING = 0, 1
+
+
 def as_records(kind, raw):
     """View a uint8 buffer of n*msg bytes as the structured wire dtype."""
     a = np.ascontiguousarray(raw, dtype=np.uint8).reshape(-1)

@@ -163,6 +163,44 @@ typedef struct dint_cfg {
 #define DINT_CFG_TATP_EBPF (1u << 3)
 #define DINT_TATP_CHAIN_REC_BYTES 212   /* {u64 key[4]; u32 ver[4]; u8 valid[4]; u8 val[4][40]}, tatp/ebpf/kvs.h:13-19 */
 
+/*
+ * dint_cfg.flags bit 4, smallbank only (dint_create / dint_cluster_create answer DINT_EINVAL for another kind, and
+ * dint_create for n_shards > 1: place smallbank shards with txn_shards): answer as the reference's eBPF SmallBank shard
+ * server (smallbank/ebpf/shard_kern.c with shard_user.c) instead of its UDP server (smallbank/udp/server_shard.cc).
+ * The eBPF server keeps the lock units {num_ex, num_sh} (the UDP server's 4H slots, lock_hash = h % 4H) and a 4-slot
+ * write-back cache set per bucket of both tables (H = A*3/2/4 buckets) in XDP maps, answers the lock traffic and cache
+ * hits there, passes misses to a user-space `kvs` and installs the answer from a TC egress program.  Per request:
+ *   - kAcquireShared / kAcquireExclusive (0 / 1): a refusal (kRejectShared 8 / kRejectExclusive 10) changes nothing;
+ *     the counters are SIGNED and refuse only when > 0 (num_ex > 0; num_ex > 0 or num_sh > 0), so a count a stray
+ *     release took below zero refuses nothing (the UDP server's unsigned == 0 test refuses); a grant counts num_sh / num_ex BEFORE the cache is looked at; a hit answers kGrantShared 7
+ *     / kGrantExclusive 9 with the set's val and ver; a miss picks a victim (first invalid slot, else first clean, else
+ *     slot 0), writes a valid dirty victim back with kvs_set(key, val, ver) (which SETS the table's version to ver when
+ *     ver != 0 and increments it when ver = 0), answers from the table and installs (key, val, ver) clean;
+ *   - kReleaseShared / kReleaseExclusive (2 / 3): decrement, no floor, answer 11 / 12 (as the UDP server);
+ *   - kCommitPrim / kCommitBck (4 / 5), no lock: a hit stores val, ver + 1, marks the slot dirty and ECHOES the client's
+ *     ver (13 / 14); a miss writes a dirty victim back, then kvs_set(key, val, 0) increments the table's version, the
+ *     reply carries the TABLE'S NEW VERSION and (key, val, new ver) is installed clean;
+ *   - kCommitLog (6): appended to the 1,000,000-entry ring and answered 15 WHATEVER THE TABLE BYTE (the UDP server
+ *     answers a table >= 2 with 0xFF);
+ *   - kWarmupRead (17), never touching the lock units: a hit answers kGrantShared (7) with the set's val and ver, a miss
+ *     goes through the table as above and answers kWarmupReadAck (18);
+ *   - a table >= 2 on another type, or a type 7-16 or >= 18: answered 0xFF (DINT_EPROTO), no state change;
+ *   - a KEY THE TABLE LACKS (an acquire, commit or warm-up miss): the reference's kvs_get / kvs_set panic and the server
+ *     stops; the engine answers 0xFF, KEEPS what happened before the table lookup (the lock counter's increment, a dirty
+ *     victim's write-back) and installs nothing.
+ * Every reply is the 23-byte struct message; ord and the bytes the server does not write are echoed.  kRetry (16) and
+ * the cache set's lock word serve contention between server threads and are never produced.
+ * dint_populate inserts every account into the tables (shard_user.c:70-78, a prefix of accts_populate accounts), then
+ * serves the eBPF client's warm-up stream (smallbank/caladan/client_ebpf_shard.cc:88-169: kWarmupRead of (saving, a)
+ * then (checking, a) for every account a this shard replicates, ascending) through the tier, so the clients start on a
+ * warm cache; dint_load inserts into the tables only and leaves the cache cold, as kvs_insert does.  dint_kv_get /
+ * dint_kv_count answer from the tables, as kvs_get would (a dirty cached value is not visible there); dint_lock_state
+ * takes the reference's lock slot (dint_lock_slot).  Costs 128 bytes of HBM per bucket (2.3 GB at A = 24,000,000).
+ * Without the bit nothing is allocated and the engine answers as smallbank/udp/server_shard.cc.
+ */
+#define DINT_CFG_SMALLBANK_EBPF (1u << 4)
+#define DINT_SMALLBANK_CACHE_ENTRY_BYTES 96   /* sizeof(struct cache_entry), smallbank/ebpf/utils.h:82-89 */
+
 typedef struct dint_engine dint_engine;
 
 /* Counters since create (or the last dint_reset_stats). */
@@ -355,6 +393,13 @@ int dint_tatp_chain(dint_engine *e, int table, uint32_t bucket, void *out, uint3
  * served by the user-space path, [3] dirty victims written back, [4] slots filled, [5] chain entries allocated from
  * the pool, [6] entries reused from the bucket's freed ones, [7] entries freed, [8] allocations that failed. */
 int dint_tatp_cache_stats(dint_engine *e, uint64_t out[9]);
+/* Cache set `bucket` (fasthash64(key) % A*3/2/4) of table `table` of a smallbank engine with DINT_CFG_SMALLBANK_EBPF,
+ * as the reference's struct cache_entry (96 bytes; lock = 0). */
+int dint_smallbank_cache_set(dint_engine *e, int table, uint32_t bucket, void *out);
+/* The tier's counters since create: out[0] requests answered from the cache (hits), [1] requests served by the
+ * user-space path (misses), [2] dirty victims written back, [3] slots installed.  Missing keys count in
+ * dint_stats.errors. */
+int dint_smallbank_cache_stats(dint_engine *e, uint64_t out[4]);
 int64_t dint_kv_count(dint_engine *e, int table);
 /* lock_2pl: out = {num_ex, num_sh}; lock_fasst: {lock, ver}; tatp: {lock, 0}; smallbank: {num_ex, num_sh} */
 int dint_lock_state(dint_engine *e, int table, uint32_t slot, uint32_t out[2]);
