@@ -152,6 +152,46 @@ DINT_D void lb_store(unsigned long long* p, unsigned long long v) {
   asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
+// Two-level look-back by ONE whole warp for tile t: publishes the tile's two counts (c0, c1) in desc[t * stride] and
+// returns their sums over tiles 0 .. t-1.  (1) the tiles before t inside its group of 32 -- one window; (2) the last tile
+// of a group publishes the group's counts in gdesc[g * stride]; (3) the groups before t's -- one window per 32 groups.
+// Nothing ever waits for a prefix, only for counts, so all tiles of a wave finish together.  Tiles must be drawn in
+// index order (a ticket), so that a tile only waits for tiles that running CTAs hold.  Every word validates itself
+// (launch number `seq` + "present" bit); counts stay below 2^27.
+DINT_D uint2 lb_exclusive(unsigned long long* desc, unsigned long long* gdesc, uint32_t stride, uint32_t seq, uint32_t t,
+                          uint32_t c0, uint32_t c1) {
+  const uint32_t lane = lane_id();
+  const uint32_t g = t >> 5, j = t & 31u;
+  if (lane == 0) lb_store(desc + (size_t)t * stride, lb_pack(seq, 1, c0, c1));
+  uint32_t x0 = 0, x1 = 0;
+  if (lane < j) {                                        // (1) tiles g*32 .. t-1
+    const unsigned long long* p = desc + (size_t)(g * 32 + lane) * stride;
+    unsigned long long v;
+    do { v = lb_load(p); } while ((uint32_t)(v >> 56) != seq || ((v >> 54) & 3u) == 0);
+    x0 = (uint32_t)v & 0x7ffffffu;
+    x1 = (uint32_t)(v >> 27) & 0x7ffffffu;
+  }
+#pragma unroll
+  for (int d = 16; d; d >>= 1) { x0 += __shfl_xor_sync(0xffffffffu, x0, d); x1 += __shfl_xor_sync(0xffffffffu, x1, d); }
+  if (j == 31 && lane == 0) lb_store(gdesc + (size_t)g * stride, lb_pack(seq, 1, x0 + c0, x1 + c1));   // (2)
+  uint32_t e0 = x0, e1 = x1;
+  for (uint32_t base = 0; base < g; base += 32) {        // (3) groups 0 .. g-1
+    uint32_t y0 = 0, y1 = 0;
+    if (base + lane < g) {
+      const unsigned long long* p = gdesc + (size_t)(base + lane) * stride;
+      unsigned long long v;
+      do { v = lb_load(p); } while ((uint32_t)(v >> 56) != seq || ((v >> 54) & 3u) == 0);
+      y0 = (uint32_t)v & 0x7ffffffu;
+      y1 = (uint32_t)(v >> 27) & 0x7ffffffu;
+    }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) { y0 += __shfl_xor_sync(0xffffffffu, y0, d); y1 += __shfl_xor_sync(0xffffffffu, y1, d); }
+    e0 += y0;
+    e1 += y1;
+  }
+  return make_uint2(e0, e1);
+}
+
 // dispatch: owner bytes, stable partition into the slabs, padding, epoch flags -- one launch, one pass
 template <int KIND>
 __global__ void __launch_bounds__(kThreads, 4) k_route_dispatch(const Ctx c, const RouteArgs a) {
@@ -205,41 +245,12 @@ __global__ void __launch_bounds__(kThreads, 4) k_route_dispatch(const Ctx c, con
     }
     Cnt8 excl, total;
     block_scan_cnt8(mine, excl, total, s_w);
-    // ---- two-level look-back over published COUNTS (nothing ever waits for a prefix, so all tiles of a wave finish
-    //      together): warp k (< 4) owns descriptor word k (two shards per word).  (1) the tiles before t inside its group of
-    //      32 -- one window; (2) the last tile of a group publishes the group's counts; (3) the groups before t's -- one
-    //      window per 32 groups.  Every word validates itself (launch number + "present" bit). ----
+    // ---- look-back over the published counts (lb_exclusive): warp k (< 4) owns descriptor word k (two shards per word) ----
     if (warp_id() < 4) {
       const uint32_t k = warp_id(), lane = lane_id();
       const uint32_t c0 = cnt8_get(total, 2 * k), c1 = cnt8_get(total, 2 * k + 1);
-      const uint32_t g = t >> 5, j = t & 31u;
-      if (lane == 0) lb_store(a.desc + (size_t)t * 4 + k, lb_pack(a.seq, 1, c0, c1));
-      uint32_t x0 = 0, x1 = 0;
-      if (lane < j) {                                    // (1) tiles g*32 .. t-1
-        const unsigned long long* p = a.desc + (size_t)(g * 32 + lane) * 4 + k;
-        unsigned long long v;
-        do { v = lb_load(p); } while ((uint32_t)(v >> 56) != a.seq || ((v >> 54) & 3u) == 0);
-        x0 = (uint32_t)v & 0x7ffffffu;
-        x1 = (uint32_t)(v >> 27) & 0x7ffffffu;
-      }
-#pragma unroll
-      for (int d = 16; d; d >>= 1) { x0 += __shfl_xor_sync(0xffffffffu, x0, d); x1 += __shfl_xor_sync(0xffffffffu, x1, d); }
-      if (j == 31 && lane == 0) lb_store(a.gdesc + (size_t)g * 4 + k, lb_pack(a.seq, 1, x0 + c0, x1 + c1));   // (2)
-      uint32_t e0 = x0, e1 = x1;
-      for (uint32_t base = 0; base < g; base += 32) {    // (3) groups 0 .. g-1
-        uint32_t y0 = 0, y1 = 0;
-        if (base + lane < g) {
-          const unsigned long long* p = a.gdesc + (size_t)(base + lane) * 4 + k;
-          unsigned long long v;
-          do { v = lb_load(p); } while ((uint32_t)(v >> 56) != a.seq || ((v >> 54) & 3u) == 0);
-          y0 = (uint32_t)v & 0x7ffffffu;
-          y1 = (uint32_t)(v >> 27) & 0x7ffffffu;
-        }
-#pragma unroll
-        for (int d = 16; d; d >>= 1) { y0 += __shfl_xor_sync(0xffffffffu, y0, d); y1 += __shfl_xor_sync(0xffffffffu, y1, d); }
-        e0 += y0;
-        e1 += y1;
-      }
+      const uint2 ex = lb_exclusive(a.desc + k, a.gdesc + k, 4, a.seq, t, c0, c1);
+      const uint32_t e0 = ex.x, e1 = ex.y;
       if (lane == 0) {
         s_base[2 * k] = e0;
         s_base[2 * k + 1] = e1;

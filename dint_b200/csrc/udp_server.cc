@@ -31,7 +31,7 @@
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
 //                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
-//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf]
+//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH] [--image-out PATH]
 //
 // --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
 // the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
@@ -52,6 +52,13 @@
 // (smallbank/ebpf/shard_kern.c), with its per-bucket write-back cache sets in front of the account tables; --populate N
 // inserts N accounts and then serves the eBPF client's warm-up stream for them (smallbank/caladan/
 // client_ebpf_shard.cc:88-169), so the cache starts as the reference's clients leave it.
+//
+// --image-in PATH: start from a state image (include/dint_b200.h, "State images") instead of populating: a file written by
+// dint_image_save, or with --gpus G > 1 a directory written by dint_cluster_image_save.  Its kind and option flags must
+// be the command line's, and for tatp / smallbank with --shards G --shard-id I it must be shard I of G, else the server
+// exits with 2.  --image-out PATH: on SIGINT / SIGTERM, once the engine threads
+// have stopped and the last replies are sent, write the state to PATH (the same file / directory forms); the exit code
+// is 1 if that fails.
 //
 // --mon-port P: the reference servers' utilisation channel (tatp/udp/server_shard.cc:213-274: a thread samples the CPU
 // time of the server's cores once a second, another answers any datagram on UDP :20231 with `struct {double ucores;
@@ -82,6 +89,12 @@
 extern "C" {
 #include "../../include/dint_b200.h"
 }
+// The state-image calls bind weakly: a library that serves requests without them (the CPU stand-in of the front-end's
+// own tests) still loads; only --image-in / --image-out need them, and say so when they are missing.
+#pragma weak dint_image_open
+#pragma weak dint_image_save
+#pragma weak dint_cluster_image_open
+#pragma weak dint_cluster_image_save
 
 namespace {
 
@@ -104,12 +117,13 @@ struct Worker {
   std::thread th;
 };
 
+const char* const kKindNames[] = {"lock_2pl", "lock_fasst", "log_server", "store", "tatp", "smallbank"};
 int kind_of(const std::string& s) {
-  static const char* names[] = {"lock_2pl", "lock_fasst", "log_server", "store", "tatp", "smallbank"};
   for (int k = 0; k < 6; k++)
-    if (s == names[k]) return k;
+    if (s == kKindNames[k]) return k;
   return -1;
 }
+const char* kind_name(uint32_t k) { return kKindNames[k]; }
 
 int open_socket(const sockaddr_in& addr, bool reuseport) {
   int fd = socket(AF_INET, SOCK_DGRAM, 0);
@@ -127,7 +141,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH] [--image-out PATH]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -137,7 +151,7 @@ int main(int argc, char** argv) {
   unsigned n_sock = std::thread::hardware_concurrency() / 2;
   if (n_sock < 1) n_sock = 1;
   if (n_sock > 8) n_sock = 8;                         // the reference runs `server 8` (exp/run_lock_fasst.sh)
-  std::string bind_addr = "0.0.0.0";
+  std::string bind_addr = "0.0.0.0", image_in, image_out;
   std::vector<int> devices;
   bool holder_keys = false, tatp_ebpf = false, smallbank_ebpf = false;
   uint32_t store_ebpf = 0;
@@ -160,6 +174,8 @@ int main(int argc, char** argv) {
     else if (a == "--linger-us") linger_us = atoi(v);
     else if (a == "--populate") populate = atoi(v);
     else if (a == "--mon-port") mon_port = atoi(v);
+    else if (a == "--image-in") image_in = v;
+    else if (a == "--image-out") image_out = v;
     else if (a == "--store-ebpf") {
       const std::string w = v;
       if (w == "wb-bloom") store_ebpf = DINT_CFG_STORE_EBPF_WB_BLOOM;
@@ -173,6 +189,11 @@ int main(int argc, char** argv) {
   if (n_sock < 1) n_sock = 1;
   if (n_sock > 64) n_sock = 64;
   if (gpus < 1 || gpus > 8 || (!devices.empty() && (int)devices.size() != gpus)) { fprintf(stderr, "bad --gpus / --devices\n"); return 2; }
+  if (!image_in.empty() && populate >= 0) { fprintf(stderr, "--image-in and --populate exclude each other\n"); return 2; }
+  if ((!image_in.empty() || !image_out.empty()) && !(dint_image_open && dint_image_save && dint_cluster_image_open && dint_cluster_image_save)) {
+    fprintf(stderr, "dint_udp_server: this libdint_b200.so has no state images (--image-in / --image-out)\n");
+    return 1;
+  }
   sockaddr_in srv{};
   srv.sin_family = AF_INET;
   if (inet_pton(AF_INET, bind_addr.c_str(), &srv.sin_addr) != 1) { fprintf(stderr, "bad --bind address\n"); return 2; }
@@ -190,7 +211,38 @@ int main(int argc, char** argv) {
   if (populate >= 0) { cfg.subs_populate = (uint32_t)populate; cfg.accts_populate = (uint32_t)populate; }   // a prefix of the reference's population
   dint_engine* eng = nullptr;
   dint_cluster* cluster = nullptr;
-  if (gpus > 1) {
+  if (!image_in.empty()) {
+    // the header's kind and dint_cfg (a state image: at byte 12 and 16; a cluster manifest: at byte 12 and 24)
+    const bool dir = gpus > 1;
+    FILE* f = fopen(dir ? (image_in + "/manifest").c_str() : image_in.c_str(), "rb");
+    uint8_t hdr[104] = {0};
+    const size_t got = f ? fread(hdr, 1, sizeof hdr, f) : 0;
+    if (f) fclose(f);
+    uint32_t img_kind = 0;
+    dint_cfg img_cfg{};
+    memcpy(&img_kind, hdr + 12, 4);
+    memcpy(&img_cfg, hdr + (dir ? 24 : 16), sizeof img_cfg);
+    if (got == sizeof hdr && ((int)img_kind != kind || img_cfg.flags != cfg.flags)) {
+      fprintf(stderr, "dint_udp_server: %s holds a %s server with option flags 0x%x; the command line asks for %s with 0x%x\n",
+              image_in.c_str(), img_kind < 6 ? kind_name(img_kind) : "unknown", img_cfg.flags, argv[1], cfg.flags);
+      return 2;
+    }
+    // server_shard <id> of a G-shard deployment (--shards / --shard-id): the image must be that shard's (txn_shards 0 and
+    // 1 both mean "every key")
+    auto placement = [](uint32_t g) { return g > 1 ? g : 1u; };
+    if (got == sizeof hdr && !dir && by_dst &&
+        (placement(img_cfg.txn_shards) != placement(shards) || (placement(shards) > 1 && img_cfg.txn_shard_id != shard_id))) {
+      fprintf(stderr, "dint_udp_server: %s holds shard %u of %u; the command line asks for shard %u of %u\n", image_in.c_str(),
+              img_cfg.txn_shard_id, placement(img_cfg.txn_shards), shard_id, placement(shards));
+      return 2;
+    }
+    const int rc = dir ? dint_cluster_image_open(image_in.c_str(), gpus, devices.empty() ? nullptr : devices.data(), 0, &cluster)
+                       : dint_image_open(image_in.c_str(), device, &eng);
+    if (rc != DINT_OK) {
+      fprintf(stderr, "dint_udp_server: opening the image failed: %s\n", dint_last_error());
+      return 1;
+    }
+  } else if (gpus > 1) {
     if (dint_cluster_create(kind, &cfg, gpus, devices.empty() ? nullptr : devices.data(), 0, &cluster) != DINT_OK ||
         dint_cluster_populate(cluster) != DINT_OK) {
       fprintf(stderr, "dint_udp_server: dint_cluster_create/populate failed: %s\n", dint_last_error());
@@ -307,9 +359,13 @@ int main(int argc, char** argv) {
         x.n = keep;
         x.state = Worker::READY;
         cv_engine.notify_one();
-        // (bounded waits: the signal handler only stores the flag, so a wakeup may be missed -- never a hang)
-        while (!cv_workers.wait_for(lk, std::chrono::milliseconds(100), [&] { return x.state == Worker::DONE || g_stop.load(); })) {}
-        if (x.state != Worker::DONE) return;
+        // (bounded waits: the signal handler only stores the flag, so a wakeup may be missed -- never a hang).  On a stop,
+        // a batch no engine thread has taken is withdrawn, unserved; one that was taken is waited for and answered, so
+        // that everything the state holds (and an --image-out saves) has been replied to.
+        while (!cv_workers.wait_for(lk, std::chrono::milliseconds(100), [&] {
+          return x.state == Worker::DONE || (g_stop.load() && x.state == Worker::READY);
+        })) {}
+        if (x.state != Worker::DONE) { x.state = Worker::FILLING; return; }
         x.state = Worker::FILLING;
       }
       // ---- send (replaces net_send): every reply goes back to the address, and from the socket, its request came to ----
@@ -469,7 +525,13 @@ int main(int argc, char** argv) {
   if (mon_sampler.joinable()) mon_sampler.join();
   if (mon_server.joinable()) mon_server.join();
   if (mon_fd >= 0) close(mon_fd);
+  int exit_code = 0;
+  if (!image_out.empty()) {                           // every engine thread has stopped and every reply was sent
+    const int rc = cluster ? dint_cluster_image_save(cluster, image_out.c_str()) : dint_image_save(eng, image_out.c_str());
+    if (rc != DINT_OK) { fprintf(stderr, "dint_udp_server: writing the image failed: %s\n", dint_last_error()); exit_code = 1; }
+    else fprintf(stderr, "dint_udp_server: state image written to %s\n", image_out.c_str());
+  }
   if (cluster) dint_cluster_destroy(cluster);
   if (eng) dint_destroy(eng);
-  return 0;
+  return exit_code;
 }

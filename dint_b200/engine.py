@@ -76,7 +76,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -145,6 +145,11 @@ def lib():
     L.dint_snapshot_create.restype = i32; L.dint_snapshot_create.argtypes = [vp, C.POINTER(vp)]
     L.dint_snapshot_restore.restype = i32; L.dint_snapshot_restore.argtypes = [vp, vp]
     L.dint_snapshot_destroy.restype = None; L.dint_snapshot_destroy.argtypes = [vp]
+    L.dint_image_save.restype = i32; L.dint_image_save.argtypes = [vp, C.c_char_p]
+    L.dint_image_open.restype = i32; L.dint_image_open.argtypes = [C.c_char_p, i32, C.POINTER(vp)]
+    L.dint_cluster_image_save.restype = i32; L.dint_cluster_image_save.argtypes = [vp, C.c_char_p]
+    L.dint_cluster_image_open.restype = i32; L.dint_cluster_image_open.argtypes = [C.c_char_p, i32, C.POINTER(i32), u64, C.POINTER(vp)]
+    L.dint_image_times.restype = i32; L.dint_image_times.argtypes = [C.POINTER(C.c_double)]
     L.dint_shard_destroy.restype = None; L.dint_shard_destroy.argtypes = [vp]
     L.dint_shard_submit_many.restype = i32; L.dint_shard_submit_many.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(vp), u64, C.POINTER(vp), vp]
     L.dint_shard_flags.restype = i32; L.dint_shard_flags.argtypes = [vp, C.POINTER(u32)]
@@ -211,6 +216,32 @@ def default_cfg(kind, **over):
         else:
             setattr(cfg, k, v)
     return cfg
+
+
+IMAGE_HEADER_BYTES = 144          # include/dint_b200.h, "State images"
+CLUSTER_MANIFEST_BYTES = 104
+
+
+def read_image_header(path):
+    """The header of a state image (or, for a directory, of its cluster manifest): kind, cfg, and for a file the
+    saved KV capacities and region count."""
+    if os.path.isdir(path):
+        with open(os.path.join(path, "manifest"), "rb") as f:
+            b = f.read(CLUSTER_MANIFEST_BYTES)
+        kind, shards = np.frombuffer(b, "<u4", 2, 12)
+        return {"magic": b[:8], "kind": int(kind), "shards": int(shards), "cfg": DintCfg.from_buffer_copy(b, 24)}
+    with open(path, "rb") as f:
+        b = f.read(IMAGE_HEADER_BYTES)
+    version, kind = np.frombuffer(b, "<u4", 2, 8)
+    return {"magic": b[:8], "version": int(version), "kind": int(kind), "cfg": DintCfg.from_buffer_copy(b, 16),
+            "n_regions": int(np.frombuffer(b, "<u4", 1, 92)[0]), "kv_capacity": [int(x) for x in np.frombuffer(b, "<u8", 5, 96)]}
+
+
+def image_times():
+    """Seconds spent by this thread's last image call: wall, pack / unpack kernels, copies, file (dint_image_times)."""
+    out = (C.c_double * 4)()
+    lib().dint_image_times(out)
+    return {"wall_s": out[0], "kernel_s": out[1], "copy_s": out[2], "file_s": out[3]}
 
 
 class PinnedBuffer:
@@ -414,6 +445,24 @@ class Engine:
 
     def free_snapshot(self, snap):
         lib().dint_snapshot_destroy(snap)
+
+    def save_image(self, path):
+        """Write the whole server state to the image file `path` (dint_image_save; waits for the engine to be idle)."""
+        rc = lib().dint_image_save(self.h, os.fsencode(path))
+        if rc != 0:
+            raise DintError(rc, f"dint_image_save({path})")
+
+    @classmethod
+    def open_image(cls, path, device=0):
+        """A new engine on `device` holding the state saved in the image file `path` (dint_image_open)."""
+        h = C.c_void_p()
+        rc = lib().dint_image_open(os.fsencode(path), device, C.byref(h))
+        if rc != 0:
+            raise DintError(rc, f"dint_image_open({path})")
+        hdr = read_image_header(path)
+        e = cls.__new__(cls)
+        e.kind, e.msg, e.cfg, e.device, e.h = hdr["kind"], MSG_SIZE[hdr["kind"]], hdr["cfg"], device, h
+        return e
 
     def sync(self, check=True):
         rc = lib().dint_sync(self.h)
@@ -637,6 +686,33 @@ class GpuCluster:
 
     def overflow_retries(self):
         return int(lib().dint_cluster_overflow_retries(self.h))
+
+    def save_image(self, path):
+        """Write every shard's state to directory `path`: a manifest and one image per shard (dint_cluster_image_save)."""
+        rc = lib().dint_cluster_image_save(self.h, os.fsencode(path))
+        if rc != 0:
+            raise DintError(rc, f"dint_cluster_image_save({path})")
+
+    @classmethod
+    def open_image(cls, path, devices=None, max_batch=0):
+        """A new cluster holding the state saved in directory `path` (dint_cluster_image_open); one shard per entry of
+        `devices` (default: as many shards as were saved, on devices 0..G-1)."""
+        if devices is not None:
+            n = len(devices)
+        else:                                   # as many shards as were saved; an unreadable manifest is the C call's to refuse
+            try:
+                n = read_image_header(path)["shards"]
+            except (OSError, ValueError):
+                n = 0
+        dv = (C.c_int * n)(*devices) if devices is not None else None
+        h = C.c_void_p()
+        rc = lib().dint_cluster_image_open(os.fsencode(path), n, dv, max_batch, C.byref(h))
+        if rc != 0:
+            raise DintError(rc, f"dint_cluster_image_open({path})")
+        hdr = read_image_header(path)
+        cl = cls.__new__(cls)
+        cl.kind, cl.msg, cl.G, cl.cfg, cl.h = hdr["kind"], MSG_SIZE[hdr["kind"]], n, hdr["cfg"], h
+        return cl
 
     def engine(self, shard):
         """A non-owning Engine view of one shard (state inspection)."""

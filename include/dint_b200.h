@@ -423,6 +423,58 @@ int dint_snapshot_restore(dint_snapshot *s, void *cuda_stream);
 void dint_snapshot_destroy(dint_snapshot *s);
 
 /*
+ * State images: the same state as a snapshot (the regions dint_snapshot_create copies), saved to a FILE, packed and
+ * checksummed on the device, and opened again as a new engine -- in another process, on another device, in a later
+ * session.  The reference has no counterpart (its state dies with the process).
+ *   dint_image_save: quiesces the engine as dint_snapshot_create does and writes `path`.  The file is written as
+ *     path.tmp, fsynced, renamed, and the directory fsynced, so a crash never leaves a half image under the final name.
+ *     It stages through three 64 MiB device buffers of the engine's host ring and three pinned host buffers, all
+ *     released when the call returns.  Block b+1 is packed
+ *     while block b is copied to pinned host memory and block b-1 is written.
+ *   dint_image_open: checks the header before any CUDA call, creates an engine on `device` from the saved dint_cfg with
+ *     every KV table at its saved capacity (the tombstone rehash may have doubled it since create), WITHOUT population or
+ *     warm-up, and streams read | copy | check + unpack.  The engine answers every later request as the saved one would.
+ *     Any failure returns no engine (*out = NULL):
+ *       DINT_EINVAL  bad magic or format version, unknown kind or option flag, a region size this build would lay
+ *                    out differently, or bytes after the last block;
+ *       DINT_EIO     a file that cannot be opened, a short read, an I/O error, or a checksum mismatch.
+ *     dint_last_error() names the file and, for a block, its region and block index.
+ *   dint_cluster_image_save: directory `dir` (created if missing) holds shard-<r>.img of every shard and, written last,
+ *     `manifest` {magic "DINTCLU1", u32 version, kind, shards, 0, the dint_cfg the cluster was created from, u32 0}.
+ *     An earlier manifest in `dir` is removed (and the removal made durable) before the first shard image is replaced,
+ *     so a save that stops part-way leaves a directory that dint_cluster_image_open refuses, never one whose shards
+ *     were saved at different moments.
+ *   dint_cluster_image_open: n_gpus must equal the manifest's shard count, and every shard file must exist; devices and
+ *     max_batch as dint_cluster_create (all ordinals distinct, or all the same).
+ *   A one-process-per-GPU deployment (dint_b200/shard.py) saves and opens each rank's engine with dint_image_save /
+ *     dint_image_open and then calls dint_shard_create as usual.
+ *   dint_image_times: the last image call of this thread, in seconds: [0] wall, [1] pack / unpack kernels (CUDA events),
+ *     [2] device <-> host copies (CUDA events), [3] file reads and writes (host clock).
+ * Not part of an image: dint_stats and the cache tiers' statistics (counters), client state (dint_clients,
+ * dint_txn_clients, dint_cluster_clients) and per-call scratch (clean at every call boundary).
+ *
+ * File layout, little-endian, format version 1:
+ *   header (144 bytes): char magic[8] = "DINTIMG1"; u32 version; u32 kind; dint_cfg cfg, 76 bytes, flags included;
+ *     u32 n_regions; u64 kv_capacity[5] (entries of every KV table at save time, 0 past n_tables); u32 tpool_cap (the
+ *     eBPF TATP chain pool's entries); u32 n_tables;
+ *   n_regions records of 24 bytes: {u32 index; u32 0; u64 raw bytes; u64 blocks = ceil(raw bytes / 64 MiB)};
+ *   then the blocks of every region in order.  A region is cut into 64 MiB raw blocks, the last one shorter.  A block
+ *   of B raw bytes has L = ceil(B / 128) lines and is stored as:
+ *     u32 bitmap[ceil(L / 128) * 4]   bit i of word w = line 32 w + i holds a non-zero byte (padding words are 0);
+ *     the lines whose bit is set, in order, 128 bytes each; a partial last line (B % 128 != 0) keeps only its B % 128
+ *       in-range bytes;
+ *     u64 checksum: the sum mod 2^64 of fasthash64(word, 4 bytes, seed 2 w) over every bitmap word w and
+ *       fasthash64(line, 128 bytes zero-padded, seed 2 i + 1) over every stored line i (its index in the block).  The
+ *       sum does not depend on the order of the device's reduction; it detects corruption and is no defence against an
+ *       attacker.
+ */
+int dint_image_save(dint_engine *e, const char *path);
+int dint_image_open(const char *path, int device, dint_engine **out);
+int dint_cluster_image_save(dint_cluster *c, const char *dir);
+int dint_cluster_image_open(const char *dir, int n_gpus, const int *devices, uint64_t max_batch, dint_cluster **out);
+int dint_image_times(double out[4]);
+
+/*
  * lock_2pl, lock_fasst, log_server and store closed-loop clients ON the GPU (SURVEY.md section 8(f) rank 2).  The
  * reference's clients are Caladan uthreads on other machines (lock_2pl/caladan/client.cc:181-230,
  * lock_fasst/caladan/client.cc:183-280, store/caladan/client_udp.cc:135-208; trace shapes lock_2pl/caladan/
