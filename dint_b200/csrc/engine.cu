@@ -23,6 +23,7 @@
 #include "clients.cuh"
 #include "txn_clients.cuh"
 #include "image.cuh"
+#include "reshard.cuh"
 
 using namespace dint;
 
@@ -401,7 +402,7 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
       ProfScope ps(e, s, KT_LOAD);
       with_kind(exec_kind(e), [&](auto k) {
         constexpr int K = decltype(k)::value;
-        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK || K == K_SMALLBANK_EBPF) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N);
+        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK || K == K_SMALLBANK_EBPF) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N, 1u, 0u);
         return DINT_OK;
       });
     }
@@ -2281,9 +2282,113 @@ void dint_cluster_destroy(dint_cluster* cl) {
 
 }  // extern "C"
 
-// dint_cluster_create, or with image_dir dint_cluster_image_open: then shard r's engine is opened from its image
+// ---- re-sharding (dint_cluster_reshard; reshard.cuh has the ownership arithmetic) ----------------------------------
+static thread_local double g_reshard_times[3];       // dint_reshard_times: wall, re-shard kernels, count + allocation (s)
+struct ReshardFrom {
+  const dint_cluster* src = nullptr;
+  std::vector<uint64_t> keys;                        // store: the live keys each destination shard receives
+};
+
+// counts, per destination shard of G2, the live keys of every source table (one small copy per source shard)
+static int reshard_count_keys(ReshardFrom& f, uint32_t G2) {
+  const dint_cluster* src = f.src;
+  f.keys.assign(G2, 0);
+  if (src->kind != DINT_STORE) return DINT_OK;
+  for (uint32_t r = 0; r < src->G; r++) {
+    const dint_engine* e = src->eng[r];
+    CU(cudaSetDevice(e->device));
+    unsigned long long* d = nullptr;
+    unsigned long long h[kMaxShards] = {0};
+    CU(cudaMalloc(&d, sizeof h));
+    cudaError_t ce = cudaMemset(d, 0, sizeof h);
+    if (ce == cudaSuccess) {
+      k_kv_owner_count<<<e->sms * 4, kThreads>>>(e->ctx.tbl[0], G2, d);
+      ce = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
+    }
+    cudaFree(d);
+    if (ce != cudaSuccess) return set_err(DINT_EIO, "re-shard key count", ce);
+    for (uint32_t j = 0; j < G2; j++) f.keys[j] += h[j];
+  }
+  return DINT_OK;
+}
+
+// Destination shard j of G2 on `device`, with configuration c: created as dint_create would (a store table at least
+// large enough to keep the keys it receives at <= 35 % load, so kv_maintain leaves it as it is), then filled from the
+// source shards by the kernels of reshard.cuh on its own stream.
+static int reshard_engine(const ReshardFrom& f, uint32_t j, uint32_t G2, dint_cfg c, int device, dint_engine** out) {
+  const dint_cluster* src = f.src;
+  *out = nullptr;
+  double t0 = img_now();
+  if (src->kind == DINT_STORE) {
+    KvPlan P;
+    if (kv_plan(DINT_STORE, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
+    uint32_t lg = P.lg[0];
+    while (lg <= 34 && f.keys[j] * 20 > (7ULL << lg)) lg++;
+    if (lg > 34) return set_errf(DINT_EINVAL, "re-shard: shard %u would receive %llu keys", j, (unsigned long long)f.keys[j]);
+    c.kv_capacity_log2[0] = lg;
+  }
+  dint_engine* e = nullptr;
+  { int rc = dint_create(src->kind, &c, device, &e); if (rc) return rc; }
+  struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
+  for (uint32_t r = 0; r < src->G; r++)                // the kernels read the source shards' arrays where they are
+    if (src->dev[r] != device) {
+      int can = 0;
+      cudaDeviceCanAccessPeer(&can, device, src->dev[r]);
+      if (!can) return set_err(DINT_ENODEV, "GPUs without peer access");
+      cudaError_t ce = cudaDeviceEnablePeerAccess(src->dev[r], 0);
+      if (ce != cudaSuccess && ce != cudaErrorPeerAccessAlreadyEnabled) return set_err(DINT_EIO, "cudaDeviceEnablePeerAccess", ce);
+      cudaGetLastError();
+    }
+  g_reshard_times[2] += img_now() - t0;
+  const Ctx& d = e->ctx;
+  const cudaStream_t s = e->stream;
+  ReshardArgs a{};
+  a.G = src->G; a.G2 = G2; a.j = j; a.src_div = make_fastmod(src->G);
+  a.n_local = (uint32_t)e->total_groups;
+  a.n_global = e->kind == DINT_STORE ? e->kv[0].hash_size : e->cfg.lock_slots;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  struct Events { cudaEvent_t* ev; ~Events() { for (int i = 0; i < 2; i++) if (ev[i]) cudaEventDestroy(ev[i]); } } evs{ev};
+  for (cudaEvent_t& x : ev) CU(cudaEventCreate(&x));
+  CU(cudaEventRecord(ev[0], s));
+  const int grid = e->sms * 4;
+  if (e->kind == DINT_LOCK2PL) {
+    for (uint32_t r = 0; r < src->G; r++) a.src[r] = (uint64_t)src->eng[r]->ctx.cnt2;
+    a.dst = d.cnt2;
+    k_reshard_lock<K_LOCK2PL><<<grid, kThreads, 0, s>>>(a);
+  } else if (e->kind == DINT_FASST) {
+    for (uint32_t r = 0; r < src->G; r++) { a.src[r] = (uint64_t)src->eng[r]->ctx.ver; a.src_bits[r] = (uint64_t)src->eng[r]->ctx.lockbits; }
+    a.dst = d.ver;
+    a.dst_bits = d.lockbits;
+    k_reshard_lock<K_FASST><<<grid, kThreads, 0, s>>>(a);
+  } else {
+    for (uint32_t r = 0; r < src->G; r++) k_kv_rehash<40><<<e->sms * 8, 256, 0, s>>>(src->eng[r]->ctx.tbl[0], d.tbl[0], G2, j);
+    if (d.ecache) {                                    // the eBPF tier: its sets move whole; its counters start at zero
+      for (uint32_t r = 0; r < src->G; r++) a.src[r] = (uint64_t)src->eng[r]->ctx.ecache;
+      a.dst = d.ecache;
+      k_reshard_sets<<<grid, kThreads, 0, s>>>(a);
+    }
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(ev[1], s));
+  CU(cudaEventSynchronize(ev[1]));
+  float ms = 0;
+  CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  g_reshard_times[1] += ms * 1e-3;
+  // the tables' {live, used} counters were recounted by the inserts: set up and refresh their host mirror, as
+  // dint_image_open does, so that the next call's kv_maintain decides on them
+  { int rc = kv_maintain(e, s); if (rc) return rc; }
+  { int rc = kv_publish_counts(e, s); if (rc) return rc; }
+  CU(cudaStreamSynchronize(s));
+  e->stats = dint_stats{};
+  own.e = nullptr;
+  *out = e;
+  return DINT_OK;
+}
+
+// dint_cluster_create; with image_dir dint_cluster_image_open: then shard r's engine is opened from its image; with
+// `from` dint_cluster_reshard: then shard r's engine is filled from the source cluster's shards
 static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* devices, uint64_t max_batch, const char* image_dir,
-                        dint_cluster** out) {
+                        const ReshardFrom* from, dint_cluster** out) {
   if (!out || kind < 0 || kind >= DINT_NUM_KINDS || n_gpus < 1 || n_gpus > kMaxShards) return set_err(DINT_EINVAL, "bad kind / n_gpus");
   *out = nullptr;
   const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
@@ -2327,7 +2432,9 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     else { c.n_shards = G; c.shard_id = r; }
     if (c.chunk == 0 || c.chunk < chunk_need) c.chunk = chunk_need;        // one batch of the exchange = one engine chunk
     dint_engine* e = nullptr;
-    rc = image_dir ? image_open_impl(img_shard_path(image_dir, r).c_str(), cl->dev[r], &c, &e) : dint_create(kind, &c, cl->dev[r], &e);
+    rc = image_dir ? image_open_impl(img_shard_path(image_dir, r).c_str(), cl->dev[r], &c, &e)
+         : from    ? reshard_engine(*from, r, G, c, cl->dev[r], &e)
+                   : dint_create(kind, &c, cl->dev[r], &e);
     if (rc == DINT_OK) cl->eng.push_back(e);
   }
   const uint32_t S = 3;
@@ -2371,7 +2478,7 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
 extern "C" {
 
 int dint_cluster_create(int kind, const dint_cfg* cfg, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
-  return cluster_make(kind, cfg, n_gpus, devices, max_batch, nullptr, out);
+  return cluster_make(kind, cfg, n_gpus, devices, max_batch, nullptr, nullptr, out);
 }
 
 int dint_cluster_image_save(dint_cluster* cl, const char* dir) {
@@ -2425,9 +2532,39 @@ int dint_cluster_image_open(const char* dir, int n_gpus, const int* devices, uin
     if (stat(img_shard_path(dir, r).c_str(), &st) != 0)
       return set_errf(DINT_EIO, "image %s: %s", img_shard_path(dir, r).c_str(), strerror(errno));
   }
-  const int rc = cluster_make((int)m.kind, &m.cfg, n_gpus, devices, max_batch, dir, out);
+  const int rc = cluster_make((int)m.kind, &m.cfg, n_gpus, devices, max_batch, dir, nullptr, out);
   g_img_times[0] = img_now() - t0;
   return rc;
+}
+
+int dint_cluster_reshard(dint_cluster* src, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
+  if (!src || !out) return set_err(DINT_EINVAL, "null argument");
+  *out = nullptr;
+  if (src->kind == DINT_TATP || src->kind == DINT_SMALLBANK)
+    return set_err(DINT_EINVAL, "tatp / smallbank: the shard count is the clients' replica placement (primary key % G, backups "
+                                "+1 and +2); another count moves which shard is primary for a key, so there is no one-server "
+                                "state to move");
+  if (src->kind == DINT_LOG) return set_err(DINT_EINVAL, "log_server: a record belongs to the rank that received it, no key decides ownership");
+  if (n_gpus < 1 || n_gpus > kMaxShards) return set_err(DINT_EINVAL, "bad n_gpus");
+  for (double& t : g_reshard_times) t = 0;
+  const double t0 = img_now();
+  for (uint32_t r = 0; r < src->G; r++) {              // quiesce the source, as dint_snapshot_create does
+    CU(cudaSetDevice(src->dev[r]));
+    CU(cudaDeviceSynchronize());
+  }
+  ReshardFrom f;
+  f.src = src;
+  { int rc = reshard_count_keys(f, (uint32_t)n_gpus); if (rc) return rc; }
+  g_reshard_times[2] += img_now() - t0;
+  const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, out);
+  g_reshard_times[0] = img_now() - t0;
+  return rc;
+}
+
+int dint_reshard_times(double out[3]) {
+  if (!out) return set_err(DINT_EINVAL, "null argument");
+  for (int i = 0; i < 3; i++) out[i] = g_reshard_times[i];
+  return DINT_OK;
 }
 
 int dint_cluster_populate(dint_cluster* cl) {
@@ -3046,6 +3183,7 @@ struct ClusterClientRank : RoundRank {
 struct dint_cluster_clients : RoundLoop {
   int kind = 0;
   uint64_t seed = 0;
+  dint_clients_cfg cfg{};        // the family the clients were made from (dint_cluster_clients_rebind makes new blocks of it)
   std::vector<ClusterClientRank> rk;
 };
 
@@ -3075,7 +3213,7 @@ int dint_cluster_clients_create(dint_cluster* cl, const dint_clients_cfg* cfg, d
     if (lo_of(r + 1) - lo_of(r) > cl->max_n) return set_err(DINT_EINVAL, "a rank's block of clients exceeds the cluster's max_batch");
   if (fallback_piece(cl) == 0) return set_err(DINT_EINVAL, "the cluster's max_batch must be >= 16");
   dint_cluster_clients* t = new dint_cluster_clients();
-  t->cl = cl; t->kind = cl->kind; t->msg = kMsgSize[cl->kind]; t->seed = cfg->seed; t->local = cl->kind == DINT_LOG;
+  t->cl = cl; t->kind = cl->kind; t->msg = kMsgSize[cl->kind]; t->seed = cfg->seed; t->local = cl->kind == DINT_LOG; t->cfg = *cfg;
   t->rk.resize(G);
   auto fail = [&](int code) { std::string keep = g_last_error; dint_cluster_clients_destroy(t); g_last_error = keep; return code; };
   for (uint32_t r = 0; r < G; r++) {
@@ -3104,8 +3242,9 @@ int dint_cluster_clients_create(dint_cluster* cl, const dint_clients_cfg* cfg, d
   return DINT_OK;
 }
 
-// enqueue one emission on every rank: the clients' kernel, then (except log_server) the per-owner count
-static int cluster_clients_emit(dint_cluster_clients* t, int first) {
+// enqueue one emission on every rank: the clients' kernel, then (except log_server) the per-owner count.  count_only:
+// the per-owner count of the pending round alone (after a rebind, for the new cluster's owners).
+static int cluster_clients_emit(dint_cluster_clients* t, int first, bool count_only = false) {
   dint_cluster* cl = t->cl;
   for (uint32_t r = 0; r < cl->G; r++) {
     ClusterClientRank& k = t->rk[r];
@@ -3114,8 +3253,10 @@ static int cluster_clients_emit(dint_cluster_clients* t, int first) {
     const cudaStream_t s = t->mains[r];
     const uint32_t n = k.b.cc.n_clients, blocks = (n + kThreads - 1) / kThreads;
     if (n) {
-      clients_launch(t->kind, t->seed, k.b, first != 0, s);
-      e->stats.kernel_launches++;
+      if (!count_only) {
+        clients_launch(t->kind, t->seed, k.b, first != 0, s);
+        e->stats.kernel_launches++;
+      }
       if (!t->local) {
         switch (t->kind) {
           case DINT_FASST: k_clients_owner_count<K_FASST><<<blocks, kThreads, 0, s>>>(e->ctx, k.b.req, n, k.acc, k.pub_dev); break;
@@ -3135,6 +3276,68 @@ static int cluster_clients_emit(dint_cluster_clients* t, int first) {
 int dint_cluster_clients_run(dint_cluster_clients* t, uint32_t rounds) {
   if (!t) return set_err(DINT_EINVAL, "null argument");
   return serve_rounds(*t, t->rk, rounds, [t](int first) { return cluster_clients_emit(t, first); });
+}
+
+// Clients [lo, lo + n) of block `from` copied into block `to` (first global id to_lo): the per-client state, the pending
+// round's requests and the last replies.  Arrays are per client, or [10][n_clients] rows (rk, rv).
+static int client_block_copy(int kind, const ClientBlock& from, int from_dev, const ClientBlock& to, int to_dev, uint32_t lo,
+                             uint32_t n) {
+  const uint32_t fo = lo - from.cc.id0, to_off = lo - to.cc.id0, msg = kMsgSize[kind];
+  auto cp = [&](const void* f, void* t, size_t es, size_t rows) -> int {
+    if (!f || !t) return DINT_OK;
+    for (size_t i = 0; i < rows; i++)
+      CU(cudaMemcpyPeer((uint8_t*)t + (i * to.cc.n_clients + to_off) * es, to_dev, (const uint8_t*)f + (i * from.cc.n_clients + fo) * es,
+                        from_dev, (size_t)n * es));
+    return DINT_OK;
+  };
+  int rc;
+  if ((rc = cp(from.req, to.req, msg, 1)) || (rc = cp(from.resp, to.resp, msg, 1))) return rc;
+  if ((rc = cp(from.cc.hdr, to.cc.hdr, 8, 1)) || (rc = cp(from.cc.rng, to.cc.rng, 8, 1)) || (rc = cp(from.cc.lcg, to.cc.lcg, 8, 1))) return rc;
+  if ((rc = cp(from.cc.rk, to.cc.rk, 4, 10)) || (rc = cp(from.cc.rv, to.cc.rv, 4, 10))) return rc;
+  return DINT_OK;
+}
+
+int dint_cluster_clients_rebind(dint_cluster_clients* t, dint_cluster* c) {
+  if (!t || !c) return set_err(DINT_EINVAL, "null argument");
+  if (c->kind != t->kind) return set_err(DINT_EINVAL, "the cluster serves another kind than these clients");
+  if (c->G > kMaxShards) return set_err(DINT_EINVAL, "bad shard count");
+  dint_cluster_clients* n = nullptr;
+  { int rc = dint_cluster_clients_create(c, &t->cfg, &n); if (rc) return rc; }   // refuses a max_batch below a rank's block
+  auto fail = [&](int code) { std::string keep = g_last_error; dint_cluster_clients_destroy(n); g_last_error = keep; return code; };
+  dint_cluster* old = t->cl;
+  for (uint32_t r = 0; r < old->G; r++) {              // the pending emission and any copy of it are done
+    if (cudaSetDevice(old->dev[r]) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
+      return fail(set_err(DINT_EIO, "rebind: synchronise", cudaGetLastError()));
+  }
+  // the clients move block by block: every (old rank, new rank) pair's common range of client ids
+  unsigned long long sum[8] = {0};
+  for (uint32_t r = 0; r < old->G; r++) {
+    const ClientBlock& f = t->rk[r].b;
+    unsigned long long h[8];
+    if (cudaSetDevice(old->dev[r]) != cudaSuccess || cudaMemcpy(h, f.cc.stats, sizeof h, cudaMemcpyDeviceToHost) != cudaSuccess)
+      return fail(set_err(DINT_EIO, "rebind: counters", cudaGetLastError()));
+    for (int i = 0; i < 8; i++) sum[i] += h[i];
+    for (uint32_t q = 0; q < c->G; q++) {
+      const ClientBlock& to = n->rk[q].b;
+      const uint32_t lo = std::max(f.cc.id0, to.cc.id0), hi = std::min(f.cc.id0 + f.cc.n_clients, to.cc.id0 + to.cc.n_clients);
+      if (lo < hi) { int rc = client_block_copy(t->kind, f, old->dev[r], to, c->dev[q], lo, hi - lo); if (rc) return fail(rc); }
+    }
+  }
+  // the counters carry over: dint_cluster_clients_stats sums the blocks, so the new rank 0 holds the old sums
+  if (cudaSetDevice(c->dev[0]) != cudaSuccess || cudaMemcpy(n->rk[0].b.cc.stats, sum, sizeof sum, cudaMemcpyHostToDevice) != cudaSuccess)
+    return fail(set_err(DINT_EIO, "rebind: counters", cudaGetLastError()));
+  // t takes the new blocks; n takes the old ones and releases them on the old cluster's devices
+  std::swap(t->cl, n->cl);
+  std::swap(t->rk, n->rk);
+  std::swap(t->mains, n->mains);
+  std::swap(t->t_beg, n->t_beg);
+  std::swap(t->t_end, n->t_end);
+  dint_cluster_clients_destroy(n);
+  if (t->started) {                                    // the pending round, counted for the new cluster's owners
+    int rc = cluster_clients_emit(t, 0, true);
+    if (rc) return rc;
+  }
+  return DINT_OK;
 }
 
 // out: dint_clients_stats_all's 6 words (rounds counted once, not once per rank), then rounds served in pieces

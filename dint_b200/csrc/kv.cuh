@@ -1133,19 +1133,23 @@ __global__ void __launch_bounds__(256) k_kv_load(const Ctx c, int table, const u
 }
 
 // Rehash of one table into a fresh (zeroed) array: every FULL entry moves with its version, tombstones vanish.
+// n_owners > 1 (a re-shard, reshard.cuh): only the entries whose global group (fasthash64(key) % to.lock_mod, the
+// reference's bucket) is owned by shard `owner` of n_owners move; `from` may then sit in a peer device's memory.
 template <int VALSZ>
-__global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvTable to) {
+__global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvTable to, uint32_t n_owners, uint32_t owner) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= from.cap_mask; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t* e = from.entries + (i << from.ent_shift);
     uint4 v[Ent<VALSZ>::NV];
     kv_load_entry<VALSZ>(e, v);
     if (v[0].w != ENT_FULL) continue;
     const uint64_t key = ((uint64_t)v[0].y << 32) | v[0].x;
+    const uint64_t h = fasthash64_u64(key);
+    if (n_owners > 1 && fast_mod(h, to.lock_mod) % n_owners != owner) continue;
     uint32_t w[Ent<VALSZ>::NW];
     const uint32_t* flat = (const uint32_t*)v;
 #pragma unroll
     for (int k = 0; k < Ent<VALSZ>::NW; k++) w[k] = flat[4 + k];
-    kv_insert_words<VALSZ>(to, key, fasthash64_u64(key), w, v[0].z);   // (`to` is at least as large: cannot fail)
+    kv_insert_words<VALSZ>(to, key, h, w, v[0].z);   // (`to` has room for every key it receives: cannot fail)
   }
 }
 
@@ -1211,32 +1215,31 @@ inline uint32_t next_log2(uint64_t x) {
 // kvs_init(S*3/2/4, S*3/2/4, S*15/4/4, S*15/4/4, S*45/8/4) (tatp/udp/server_shard.cc:75-79); smallbank
 // kvs_init(A*3/2/4) x2 (smallbank/udp/server_shard.cc:72-73).  The group modulus is the bucket count
 // for store and kKeysPerEntry*hash_size (lock_hash) for tatp / smallbank.
-template <typename AllocFn>
 // tatp_ebpf: the eBPF server's sizes (tatp/ebpf/utils.h:17-21: call_forwarding has S*15/4/4 buckets); its rows live in
 // chained tables (kv.cuh, K_TATP_EBPF), so the open-addressing tables are left at their minimum size, unused.
-int kv_create_tables(int kind, const dint_cfg& cf, Ctx& c, KvHost* kv, uint64_t* groups_out, AllocFn alloc, bool tatp_ebpf = false) {
-  const uint64_t S = cf.subs_sizing, Sp = cf.subs_populate, A = cf.accts_sizing, Ap = cf.accts_populate;
-  uint32_t hs[kMaxTables] = {0};
-  double expect[kMaxTables] = {0};
+struct KvPlan {
   uint32_t nt = 0, valsz = 40, lock_mul = 4;
+  uint32_t hs[kMaxTables] = {0};     // bucket counts
+  uint32_t lg[kMaxTables] = {0};     // log2 capacities a shard of `cf` is created with
+};
+inline int kv_plan(int kind, const dint_cfg& cf, bool tatp_ebpf, KvPlan& p) {
+  const uint64_t S = cf.subs_sizing, Sp = cf.subs_populate, A = cf.accts_sizing, Ap = cf.accts_populate;
+  double expect[kMaxTables] = {0};
   if (kind == DINT_STORE) {
-    nt = 1; hs[0] = (uint32_t)(S * 18 / 4); expect[0] = 12.0 * Sp; lock_mul = 1;
+    p.nt = 1; p.hs[0] = (uint32_t)(S * 18 / 4); expect[0] = 12.0 * Sp; p.lock_mul = 1;
   } else if (kind == DINT_TATP) {
-    nt = 5;
-    hs[0] = hs[1] = (uint32_t)(S * 3 / 2 / 4);
-    hs[2] = hs[3] = (uint32_t)(S * 15 / 4 / 4);
-    hs[4] = tatp_ebpf ? (uint32_t)(S * 15 / 4 / 4) : (uint32_t)(S * 45 / 8 / 4);
+    p.nt = 5;
+    p.hs[0] = p.hs[1] = (uint32_t)(S * 3 / 2 / 4);
+    p.hs[2] = p.hs[3] = (uint32_t)(S * 15 / 4 / 4);
+    p.hs[4] = tatp_ebpf ? (uint32_t)(S * 15 / 4 / 4) : (uint32_t)(S * 45 / 8 / 4);
     expect[0] = expect[1] = 1.0 * Sp; expect[2] = expect[3] = 2.5 * Sp; expect[4] = 3.75 * Sp;
   } else if (kind == DINT_SMALLBANK) {
-    nt = 2; valsz = 8;
-    hs[0] = hs[1] = (uint32_t)(A * 3 / 2 / 4);
+    p.nt = 2; p.valsz = 8;
+    p.hs[0] = p.hs[1] = (uint32_t)(A * 3 / 2 / 4);
     expect[0] = expect[1] = 1.0 * Ap;
   } else return DINT_EINVAL;
-  c.n_tables = nt;
-  uint64_t base = 0;
-  for (uint32_t t = 0; t < nt; t++) {
-    if (hs[t] == 0) return DINT_EINVAL;
-    KvTable& T = c.tbl[t];
+  for (uint32_t t = 0; t < p.nt; t++) {
+    if (p.hs[t] == 0) return DINT_EINVAL;
     uint32_t lg = tatp_ebpf ? 10 : cf.kv_capacity_log2[t];
     if (lg == 0) {
       double need = 2.0 * expect[t] / cf.n_shards * 1.05 + 1024;
@@ -1244,6 +1247,22 @@ int kv_create_tables(int kind, const dint_cfg& cf, Ctx& c, KvHost* kv, uint64_t*
       if (lg < 10) lg = 10;
     }
     if (lg > 34) return DINT_EINVAL;
+    p.lg[t] = lg;
+  }
+  return DINT_OK;
+}
+
+template <typename AllocFn>
+int kv_create_tables(int kind, const dint_cfg& cf, Ctx& c, KvHost* kv, uint64_t* groups_out, AllocFn alloc, bool tatp_ebpf = false) {
+  KvPlan P;
+  if (kv_plan(kind, cf, tatp_ebpf, P) != DINT_OK) return DINT_EINVAL;
+  const uint32_t nt = P.nt, valsz = P.valsz, lock_mul = P.lock_mul;
+  const uint32_t* hs = P.hs;
+  c.n_tables = nt;
+  uint64_t base = 0;
+  for (uint32_t t = 0; t < nt; t++) {
+    KvTable& T = c.tbl[t];
+    const uint32_t lg = P.lg[t];
     T.cap_log2 = lg;
     T.cap_mask = (1ULL << lg) - 1;
     T.ent_shift = (valsz == 40) ? 6 : 5;

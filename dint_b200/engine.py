@@ -76,7 +76,7 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_cluster_reshard", "dint_reshard_times", "dint_cluster_clients_rebind", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
     "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
@@ -150,6 +150,9 @@ def lib():
     L.dint_cluster_image_save.restype = i32; L.dint_cluster_image_save.argtypes = [vp, C.c_char_p]
     L.dint_cluster_image_open.restype = i32; L.dint_cluster_image_open.argtypes = [C.c_char_p, i32, C.POINTER(i32), u64, C.POINTER(vp)]
     L.dint_image_times.restype = i32; L.dint_image_times.argtypes = [C.POINTER(C.c_double)]
+    L.dint_cluster_reshard.restype = i32; L.dint_cluster_reshard.argtypes = [vp, i32, C.POINTER(i32), u64, C.POINTER(vp)]
+    L.dint_reshard_times.restype = i32; L.dint_reshard_times.argtypes = [C.POINTER(C.c_double)]
+    L.dint_cluster_clients_rebind.restype = i32; L.dint_cluster_clients_rebind.argtypes = [vp, vp]
     L.dint_shard_destroy.restype = None; L.dint_shard_destroy.argtypes = [vp]
     L.dint_shard_submit_many.restype = i32; L.dint_shard_submit_many.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(vp), u64, C.POINTER(vp), vp]
     L.dint_shard_flags.restype = i32; L.dint_shard_flags.argtypes = [vp, C.POINTER(u32)]
@@ -235,6 +238,14 @@ def read_image_header(path):
     version, kind = np.frombuffer(b, "<u4", 2, 8)
     return {"magic": b[:8], "version": int(version), "kind": int(kind), "cfg": DintCfg.from_buffer_copy(b, 16),
             "n_regions": int(np.frombuffer(b, "<u4", 1, 92)[0]), "kv_capacity": [int(x) for x in np.frombuffer(b, "<u8", 5, 96)]}
+
+
+def reshard_times():
+    """Seconds spent by this thread's last GpuCluster.reshard: wall, re-shard kernels (CUDA events), key count +
+    allocation of the destination (dint_reshard_times)."""
+    out = (C.c_double * 3)()
+    lib().dint_reshard_times(out)
+    return {"wall_s": out[0], "kernel_s": out[1], "count_alloc_s": out[2]}
 
 
 def image_times():
@@ -714,6 +725,19 @@ class GpuCluster:
         cl.kind, cl.msg, cl.G, cl.cfg, cl.h = hdr["kind"], MSG_SIZE[hdr["kind"]], n, hdr["cfg"], h
         return cl
 
+    def reshard(self, n_shards, devices=None, max_batch=0):
+        """A new cluster of `n_shards` shards holding this one's state (dint_cluster_reshard): it answers every later
+        request exactly as this one would.  lock_2pl / lock_fasst / store only; this cluster is not changed and stays
+        usable.  devices / max_batch as for GpuCluster; peak device memory is both clusters."""
+        dv = (C.c_int * n_shards)(*devices) if devices is not None else None
+        h = C.c_void_p()
+        rc = lib().dint_cluster_reshard(self.h, n_shards, dv, max_batch, C.byref(h))
+        if rc != 0:
+            raise DintError(rc, f"dint_cluster_reshard({KIND_NAMES[self.kind]}, {self.G} -> {n_shards})")
+        cl = GpuCluster.__new__(GpuCluster)
+        cl.kind, cl.msg, cl.G, cl.cfg, cl.h = self.kind, self.msg, n_shards, self.cfg, h
+        return cl
+
     def engine(self, shard):
         """A non-owning Engine view of one shard (state inspection)."""
         e = Engine.__new__(Engine)
@@ -871,6 +895,14 @@ class GpuClusterClients:
         if rc != 0:
             raise DintError(rc, "dint_cluster_clients_peek")
         return rq, rs
+
+    def rebind(self, cluster):
+        """Move the clients to `cluster`, a GpuCluster of the same kind (e.g. from GpuCluster.reshard): their state, the
+        pending round and the counters carry over (dint_cluster_clients_rebind).  The old cluster may then be closed."""
+        rc = lib().dint_cluster_clients_rebind(self.h, cluster.h)
+        if rc != 0:
+            raise DintError(rc, "dint_cluster_clients_rebind")
+        self.cluster = cluster
 
     def times(self):
         """Rounds timed by run(), their host wall time and the CUDA-event time of their device work (rank 0), in s."""

@@ -475,6 +475,36 @@ int dint_cluster_image_open(const char *dir, int n_gpus, const int *devices, uin
 int dint_image_times(double out[4]);
 
 /*
+ * Re-sharding: the state of a lock_2pl, lock_fasst or store cluster does not depend on its shard count G, only its layout
+ * over the shards does (shard r owns the lock slots / buckets s with s % G == r, at local index s / G).
+ *   dint_cluster_reshard: a new cluster of n_gpus shards holding src's state, which answers every later request exactly
+ *     as src would.  src is read, never changed, and stays usable.  It synchronises every source device first (a quiesce
+ *     point, like dint_snapshot_create: nothing may be in flight on src), then builds the destination as
+ *     dint_cluster_create(kind, cfg, n_gpus, devices, max_batch) would -- same exchange buffers, chunk, slab capacity and
+ *     persisting-L2 window, and the same `cfg`, so a later dint_cluster_image_save writes a manifest that
+ *     dint_cluster_image_open(dir, n_gpus, ...) accepts -- and fills every shard on its own device:
+ *       lock_2pl   {num_ex, num_sh} of every slot;
+ *       lock_fasst the version and the lock bit of every slot: a lock granted before the call is still held after it;
+ *       store      every live key with its value and version (tombstones are dropped; each destination table is at least
+ *                  as large as dint_cluster_create would make it, and large enough to keep its keys at <= 35 % load, so
+ *                  the tombstone rehash does not run on the first call); with DINT_CFG_STORE_EBPF_* every 256-byte cache
+ *                  set moves whole (keys, versions, valid and dirty masks, bloom word).
+ *     A source shard on another GPU is read over peer memory (peer access is enabled for each such pair, DINT_ENODEV
+ *     where there is none).  Statistics (dint_stats, the cache tier's counters) start at zero, as after an image open.
+ *     Peak device memory is the source plus the destination: destroy src afterwards to release it.
+ *     A key that reached a store table twice (a second eBPF kInsert of it) keeps both copies, but which one a lookup
+ *     finds may change -- the limit the tombstone rehash already has (DINT_CFG_STORE_EBPF_*, "Limit").
+ *     DINT_EINVAL and no cluster (*out = NULL): tatp and smallbank (their shard count is the clients' replica placement,
+ *     primary key % G with backups +1 and +2, so another count changes which shard is primary for a key and there is no
+ *     one-server state to move), log_server (a record belongs to the rank that received it; no key decides ownership),
+ *     n_gpus outside 1..8, and devices that are neither all distinct nor all the same.  n_gpus == G is a plain copy.
+ *   dint_reshard_times: the last dint_cluster_reshard of this thread, in seconds: [0] wall, [1] the re-shard kernels
+ *     (CUDA events, summed over the destination shards), [2] the key count and the destination engines' allocation.
+ */
+int dint_cluster_reshard(dint_cluster *src, int n_gpus, const int *devices, uint64_t max_batch, dint_cluster **out);
+int dint_reshard_times(double out[3]);
+
+/*
  * lock_2pl, lock_fasst, log_server and store closed-loop clients ON the GPU (SURVEY.md section 8(f) rank 2).  The
  * reference's clients are Caladan uthreads on other machines (lock_2pl/caladan/client.cc:181-230,
  * lock_fasst/caladan/client.cc:183-280, store/caladan/client_udp.cc:135-208; trace shapes lock_2pl/caladan/
@@ -571,6 +601,11 @@ void dint_txn_clients_destroy(dint_txn_clients *t);
  *   dint_cluster_clients_peek (test hook, synchronises): in global client order, the next round's requests / the last
  *     round's replies, n_clients * dint_msg_size(kind) bytes each.
  *   dint_cluster_clients_times: as dint_txn_clients_times.
+ *   dint_cluster_clients_rebind: move the clients to cluster c (e.g. the result of dint_cluster_reshard): their state,
+ *     the pending round's requests and the last replies are redistributed over c's ranks in contiguous blocks, across
+ *     devices if needed, and the counters carry over, so stats keep counting from where they were.  Afterwards the
+ *     clients no longer reference the old cluster, which may be destroyed.  DINT_EINVAL (the clients unchanged) for a
+ *     cluster of another kind, and when a rank's block of c exceeds c's max_batch, as at create.
  * The first round is emitted by the first run or peek call.
  */
 typedef struct dint_cluster_clients dint_cluster_clients;
@@ -579,6 +614,7 @@ int dint_cluster_clients_run(dint_cluster_clients *t, uint32_t rounds);
 int dint_cluster_clients_stats(dint_cluster_clients *t, uint64_t out[7]);
 int dint_cluster_clients_peek(dint_cluster_clients *t, void *next_req, void *last_resp);
 int dint_cluster_clients_times(dint_cluster_clients *t, double out[3]);
+int dint_cluster_clients_rebind(dint_cluster_clients *t, dint_cluster *c);
 void dint_cluster_clients_destroy(dint_cluster_clients *t);
 
 int dint_get_stats(dint_engine *e, dint_stats *s);
