@@ -24,6 +24,7 @@
 #include "txn_clients.cuh"
 #include "image.cuh"
 #include "reshard.cuh"
+#include "rebuild.cuh"
 
 using namespace dint;
 
@@ -581,6 +582,9 @@ uint32_t dint_log_entry_size(int kind) { return (kind >= 0 && kind < DINT_NUM_KI
 const char* dint_last_error(void) { return g_last_error.c_str(); }
 uint64_t dint_test_fasthash64(uint64_t x, int len) { return len == 4 ? fasthash64_u32((uint32_t)x) : fasthash64_u64(x); }
 uint32_t dint_test_fastmod(uint64_t n, uint32_t d) { FastMod f = make_fastmod(d); return fast_mod(n, f); }
+int dint_test_rebuild_source(uint64_t key, uint32_t G, uint32_t lost_mask) {
+  return G == 0 || G > kMaxShards ? -1 : rebuild_source((uint32_t)(key % G), G, lost_mask);
+}
 uint32_t dint_test_host_slices(uint64_t n, uint32_t min_slice, uint32_t max_slice, int ramp_up, uint32_t* out, uint32_t cap) {
   HostSlices sched(n, min_slice, max_slice, ramp_up != 0);
   uint32_t k = 0;
@@ -2270,7 +2274,44 @@ struct dint_cluster {
   std::vector<void*> bufs;                  // per rank: one allocation {inbox sets | return-buffer sets | signal block}
   uint64_t overflow_retries = 0;            // submit calls that met a slab overflow and served the rest in small rounds
   dint_cfg base{};                          // the configuration the shards were made from (the image manifest keeps it)
+  uint32_t txn_clients = 0;                 // dint_txn_clients attached (dint_cluster_rebuild refuses while there are any)
 };
+
+// The exchange buffers of a cluster: per rank one allocation {inbox sets | return-buffer sets | signal block}
+constexpr uint32_t kClusterSets = 3;
+static size_t cluster_region(const dint_cluster* cl) { return ((size_t)cl->G * cl->cap * kMsgSize[cl->kind] + 255) / 256 * 256; }
+static uint64_t cluster_sig_block(const dint_cluster* cl, uint32_t r) { return (uint64_t)cl->bufs[r] + 2 * kClusterSets * cluster_region(cl); }
+
+// the configuration shard r of a cluster is created with (cl->base, cap and G set)
+static dint_cfg cluster_shard_cfg(const dint_cluster* cl, uint32_t r) {
+  dint_cfg c = cl->base;
+  if (cl->by_dst) { c.n_shards = 1; c.shard_id = 0; c.txn_shards = cl->G; c.txn_shard_id = r; }
+  else { c.n_shards = cl->G; c.shard_id = r; }
+  const uint32_t chunk_need = (uint32_t)(((uint64_t)cl->G * cl->cap + kTile - 1) / kTile * kTile);
+  if (c.chunk == 0 || c.chunk < chunk_need) c.chunk = chunk_need;        // one batch of the exchange = one engine chunk
+  return c;
+}
+
+// one shard context per rank over the cluster's exchange buffers, engine r = eng[r]; every epoch starts at 0, so the
+// signal blocks must be zero before the first batch
+static int cluster_ranks(const dint_cluster* cl, const std::vector<dint_engine*>& eng, std::vector<dint_shard_ctx*>& out) {
+  const uint32_t G = cl->G, S = kClusterSets;
+  const size_t region = cluster_region(cl);
+  for (uint32_t r = 0; r < G; r++) {
+    dint_peer_ptrs in[kMaxSets]{}, rb[kMaxSets]{}, sig{};
+    for (uint32_t s = 0; s < S; s++)
+      for (uint32_t o = 0; o < G; o++) {
+        in[s].p[o] = (uint64_t)cl->bufs[o] + (2 * s) * region;
+        rb[s].p[o] = (uint64_t)cl->bufs[o] + (2 * s + 1) * region;
+      }
+    for (uint32_t o = 0; o < G; o++) sig.p[o] = cluster_sig_block(cl, o);
+    dint_shard_ctx* c = nullptr;
+    int rc = shard_make(eng[r], G, r, cl->cap, S, in, rb, &sig, cl->max_n, cl->shared_device, &c);
+    if (rc) return rc;
+    out.push_back(c);
+  }
+  return DINT_OK;
+}
 
 void dint_cluster_destroy(dint_cluster* cl) {
   if (!cl) return;
@@ -2288,6 +2329,18 @@ struct ReshardFrom {
   const dint_cluster* src = nullptr;
   std::vector<uint64_t> keys;                        // store: the live keys each destination shard receives
 };
+
+// lets `device` (the current device) read `peer`'s memory; nothing to do when they are the same
+static int peer_enable(int device, int peer) {
+  if (peer == device) return DINT_OK;
+  int can = 0;
+  cudaDeviceCanAccessPeer(&can, device, peer);
+  if (!can) return set_err(DINT_ENODEV, "GPUs without peer access");
+  cudaError_t ce = cudaDeviceEnablePeerAccess(peer, 0);
+  if (ce != cudaSuccess && ce != cudaErrorPeerAccessAlreadyEnabled) return set_err(DINT_EIO, "cudaDeviceEnablePeerAccess", ce);
+  cudaGetLastError();
+  return DINT_OK;
+}
 
 // counts, per destination shard of G2, the live keys of every source table (one small copy per source shard)
 static int reshard_count_keys(ReshardFrom& f, uint32_t G2) {
@@ -2322,23 +2375,17 @@ static int reshard_engine(const ReshardFrom& f, uint32_t j, uint32_t G2, dint_cf
   if (src->kind == DINT_STORE) {
     KvPlan P;
     if (kv_plan(DINT_STORE, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
-    uint32_t lg = P.lg[0];
-    while (lg <= 34 && f.keys[j] * 20 > (7ULL << lg)) lg++;
+    const uint32_t lg = kv_fit_log2(P.lg[0], f.keys[j]);
     if (lg > 34) return set_errf(DINT_EINVAL, "re-shard: shard %u would receive %llu keys", j, (unsigned long long)f.keys[j]);
     c.kv_capacity_log2[0] = lg;
   }
   dint_engine* e = nullptr;
   { int rc = dint_create(src->kind, &c, device, &e); if (rc) return rc; }
   struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
-  for (uint32_t r = 0; r < src->G; r++)                // the kernels read the source shards' arrays where they are
-    if (src->dev[r] != device) {
-      int can = 0;
-      cudaDeviceCanAccessPeer(&can, device, src->dev[r]);
-      if (!can) return set_err(DINT_ENODEV, "GPUs without peer access");
-      cudaError_t ce = cudaDeviceEnablePeerAccess(src->dev[r], 0);
-      if (ce != cudaSuccess && ce != cudaErrorPeerAccessAlreadyEnabled) return set_err(DINT_EIO, "cudaDeviceEnablePeerAccess", ce);
-      cudaGetLastError();
-    }
+  for (uint32_t r = 0; r < src->G; r++) {             // the kernels read the source shards' arrays where they are
+    int rc = peer_enable(device, src->dev[r]);
+    if (rc) return rc;
+  }
   g_reshard_times[2] += img_now() - t0;
   const Ctx& d = e->ctx;
   const cudaStream_t s = e->stream;
@@ -2385,10 +2432,123 @@ static int reshard_engine(const ReshardFrom& f, uint32_t j, uint32_t G2, dint_cf
   return DINT_OK;
 }
 
+// ---- rebuilding lost tatp / smallbank shards (dint_cluster_rebuild; rebuild.cuh has the placement arithmetic) -----
+static thread_local double g_rebuild_times[3];       // dint_rebuild_times: wall, rebuild kernels, count + allocation (s)
+
+static std::string mask_names(uint32_t mask) {
+  std::string s;
+  for (uint32_t r = 0; r < 32; r++)
+    if ((mask >> r) & 1u) s += (s.empty() ? "" : ", ") + std::to_string(r);
+  return "{" + s + "}";
+}
+
+// DINT_EINVAL, with the reason, unless the shards of `lost` of a G-shard cluster of this kind and configuration can be
+// rebuilt from the others
+static int rebuild_check(int kind, const dint_cfg& cfg, uint32_t G, uint32_t lost) {
+  if (kind != DINT_TATP && kind != DINT_SMALLBANK)
+    return set_err(DINT_EINVAL, "rebuild: lock_2pl, lock_fasst, store and log_server clusters keep no replicas");
+  if (cfg.flags & (DINT_CFG_TATP_EBPF | DINT_CFG_SMALLBANK_EBPF))
+    return set_err(DINT_EINVAL, "rebuild: the eBPF cache tiers hold dirty and cache-only rows whose wire-visible versions depend on "
+                                "each shard's own hit history, so no peer's copy is that shard's state");
+  if (G < 3) return set_err(DINT_EINVAL, "rebuild: a one-shard cluster has no replica to rebuild from");
+  if (lost == 0 || (lost >> G) != 0) return set_errf(DINT_EINVAL, "rebuild: lost mask 0x%x is empty or names shards outside [0, %u)", lost, G);
+  for (uint32_t p = 0; p < G; p++)
+    if (rebuild_source(p, G, lost) < 0)
+      return set_errf(DINT_EINVAL, "rebuild: losing shards %s leaves the keys k with k %% %u == %u without a replica",
+                      mask_names(lost).c_str(), G, p);
+  return DINT_OK;
+}
+
+struct RebuildFrom {
+  std::vector<dint_engine*> src;                     // per shard: the engine read (nullptr where lost)
+  uint32_t G = 0, lost = 0;
+  uint64_t keys[kMaxShards][kMaxTables] = {};        // the rows each lost shard receives, per table
+  // may shard s hold keys of lost shard d: within two positions of it, either way round
+  bool near(uint32_t s, uint32_t d) const { const uint32_t a = (s + G - d) % G; return a <= 2 || a >= G - 2; }
+  RebuildKeep keep(uint32_t s, uint32_t d) const { return RebuildKeep{make_fastmod(G), G, lost, s, d}; }
+};
+
+// f.src / G / lost, then every surviving source's rows per (table, lost shard): one small copy per source shard
+static int rebuild_prepare(RebuildFrom& f, const std::vector<dint_engine*>& eng, uint32_t G, uint32_t lost) {
+  f.src = eng; f.G = G; f.lost = lost;
+  for (uint32_t r = 0; r < G; r++) if ((lost >> r) & 1u) f.src[r] = nullptr;
+  for (uint32_t s = 0; s < G; s++) {
+    const dint_engine* e = f.src[s];
+    bool reads = false;
+    for (uint32_t d = 0; d < G; d++) reads |= ((lost >> d) & 1u) && f.near(s, d);
+    if (!e || !reads) continue;
+    CU(cudaSetDevice(e->device));
+    unsigned long long* d = nullptr;
+    unsigned long long h[kMaxTables][kMaxShards] = {};
+    CU(cudaMalloc(&d, sizeof h));
+    cudaError_t ce = cudaMemset(d, 0, sizeof h);
+    for (uint32_t t = 0; t < e->ctx.n_tables && ce == cudaSuccess; t++) {
+      k_rebuild_count<<<e->sms * 4, kThreads>>>(e->ctx.tbl[t], f.keep(s, 0), d + t * kMaxShards);
+      ce = cudaGetLastError();
+    }
+    if (ce == cudaSuccess) ce = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    if (ce != cudaSuccess) return set_err(DINT_EIO, "rebuild row count", ce);
+    for (uint32_t t = 0; t < kMaxTables; t++)
+      for (uint32_t j = 0; j < G; j++) f.keys[j][t] += h[t][j];
+  }
+  return DINT_OK;
+}
+
+// Lost shard j on `device`, with configuration c: created as dint_create would (every table at least large enough to
+// keep the rows it receives at <= 35 % load, so kv_maintain leaves it as it is), then filled from the surviving
+// sources within two positions of it by k_rebuild_rows on its own stream.  Lock words, holder keys, the log ring and the
+// statistics are those of a new engine.
+static int rebuild_engine(const RebuildFrom& f, uint32_t j, int kind, dint_cfg c, int device, dint_engine** out) {
+  *out = nullptr;
+  double t0 = img_now();
+  KvPlan P;
+  if (kv_plan(kind, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
+  for (uint32_t t = 0; t < P.nt; t++) {
+    const uint32_t lg = kv_fit_log2(P.lg[t], f.keys[j][t]);
+    if (lg > 34) return set_errf(DINT_EINVAL, "rebuild: shard %u table %u would receive %llu rows", j, t, (unsigned long long)f.keys[j][t]);
+    c.kv_capacity_log2[t] = lg;
+  }
+  dint_engine* e = nullptr;
+  { int rc = dint_create(kind, &c, device, &e); if (rc) return rc; }
+  struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
+  for (uint32_t s = 0; s < f.G; s++)
+    if (f.src[s] && f.near(s, j)) { int rc = peer_enable(device, f.src[s]->device); if (rc) return rc; }
+  g_rebuild_times[2] += img_now() - t0;
+  const cudaStream_t st = e->stream;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  struct Events { cudaEvent_t* ev; ~Events() { for (int i = 0; i < 2; i++) if (ev[i]) cudaEventDestroy(ev[i]); } } evs{ev};
+  for (cudaEvent_t& x : ev) CU(cudaEventCreate(&x));
+  CU(cudaEventRecord(ev[0], st));
+  for (uint32_t s = 0; s < f.G; s++) {
+    if (!f.src[s] || !f.near(s, j)) continue;
+    const Ctx& from = f.src[s]->ctx;
+    for (uint32_t t = 0; t < e->ctx.n_tables; t++) {
+      if (kind == DINT_SMALLBANK) k_rebuild_rows<8><<<e->sms * 8, 256, 0, st>>>(from.tbl[t], e->ctx.tbl[t], f.keep(s, j));
+      else k_rebuild_rows<40><<<e->sms * 8, 256, 0, st>>>(from.tbl[t], e->ctx.tbl[t], f.keep(s, j));
+    }
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(ev[1], st));
+  CU(cudaEventSynchronize(ev[1]));
+  float ms = 0;
+  CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  g_rebuild_times[1] += ms * 1e-3;
+  { int rc = kv_maintain(e, st); if (rc) return rc; }     // the host mirror of {live, used}, as reshard_engine
+  { int rc = kv_publish_counts(e, st); if (rc) return rc; }
+  CU(cudaStreamSynchronize(st));
+  e->stats = dint_stats{};
+  own.e = nullptr;
+  *out = e;
+  return DINT_OK;
+}
+
 // dint_cluster_create; with image_dir dint_cluster_image_open: then shard r's engine is opened from its image; with
-// `from` dint_cluster_reshard: then shard r's engine is filled from the source cluster's shards
+// `from` dint_cluster_reshard: then shard r's engine is filled from the source cluster's shards.  With image_dir and
+// `rebuild` (dint_cluster_image_open_rebuild): the shards of *rebuild (known missing) and those whose image fails with
+// DINT_EIO are rebuilt from the others once those are open; *rebuild is then set to every shard rebuilt.
 static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* devices, uint64_t max_batch, const char* image_dir,
-                        const ReshardFrom* from, dint_cluster** out) {
+                        const ReshardFrom* from, uint32_t* rebuild, dint_cluster** out) {
   if (!out || kind < 0 || kind >= DINT_NUM_KINDS || n_gpus < 1 || n_gpus > kMaxShards) return set_err(DINT_EINVAL, "bad kind / n_gpus");
   *out = nullptr;
   const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
@@ -2411,7 +2571,6 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     for (int r = 1; r < n_gpus; r++)
       if (cl->dev[r] != cl->dev[0]) { delete cl; return set_err(DINT_EINVAL, "devices must be all distinct or all the same"); }
   const uint32_t G = cl->G;
-  const uint32_t msg = kMsgSize[kind];
   if (max_batch == 0) max_batch = 1u << 18;
   cl->max_n = max_batch;
   {
@@ -2425,27 +2584,37 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
   int rc = DINT_OK;
   dint_cfg& base = cl->base;
   if (cfg) base = *cfg; else dint_default_cfg(kind, &base);
-  const uint32_t chunk_need = (uint32_t)(((uint64_t)G * cl->cap + kTile - 1) / kTile * kTile);
+  uint32_t failed = 0;                                  // rebuild: shards whose image failed with DINT_EIO
   for (uint32_t r = 0; r < G && rc == DINT_OK; r++) {
-    dint_cfg c = base;
-    if (by_dst) { c.n_shards = 1; c.shard_id = 0; c.txn_shards = G; c.txn_shard_id = r; }
-    else { c.n_shards = G; c.shard_id = r; }
-    if (c.chunk == 0 || c.chunk < chunk_need) c.chunk = chunk_need;        // one batch of the exchange = one engine chunk
+    const dint_cfg c = cluster_shard_cfg(cl, r);
     dint_engine* e = nullptr;
+    if (rebuild && ((*rebuild >> r) & 1u)) { failed |= 1u << r; cl->eng.push_back(nullptr); continue; }   // known missing
     rc = image_dir ? image_open_impl(img_shard_path(image_dir, r).c_str(), cl->dev[r], &c, &e)
          : from    ? reshard_engine(*from, r, G, c, cl->dev[r], &e)
                    : dint_create(kind, &c, cl->dev[r], &e);
+    if (rc == DINT_EIO && rebuild) {                    // a short, unreadable or corrupt image: rebuilt below
+      failed |= 1u << r;
+      rc = DINT_OK;
+    }
     if (rc == DINT_OK) cl->eng.push_back(e);
   }
-  const uint32_t S = 3;
-  const size_t region = ((size_t)G * cl->cap * msg + 255) / 256 * 256;
-  std::vector<uint64_t> base_ptr(G);
+  if (rc == DINT_OK && failed) {                        // the present shards are open: fill the failed ones from them
+    rc = rebuild_check(kind, base, G, failed);
+    if (rc) rc = set_errf(DINT_EIO, "image %s: shard image(s) %s failed and cannot be rebuilt: %s", image_dir,
+                          mask_names(failed).c_str(), g_last_error.c_str());
+    RebuildFrom f;
+    if (rc == DINT_OK) rc = rebuild_prepare(f, cl->eng, G, failed);
+    for (uint32_t r = 0; r < G && rc == DINT_OK; r++)
+      if ((failed >> r) & 1u) rc = rebuild_engine(f, r, kind, cluster_shard_cfg(cl, r), cl->dev[r], &cl->eng[r]);
+    if (rc == DINT_OK) *rebuild = failed;
+  }
+  const uint32_t S = kClusterSets;
+  const size_t region = cluster_region(cl);
   for (uint32_t r = 0; r < G && rc == DINT_OK; r++) {
     void* p = nullptr;
     if (cudaSetDevice(cl->dev[r]) != cudaSuccess || cudaMalloc(&p, 2 * S * region + 4096) != cudaSuccess) { rc = set_err(DINT_ENOMEM, "cluster buffers", cudaGetLastError()); break; }
     cudaMemset(p, 0, 2 * S * region + 4096);
     cl->bufs.push_back(p);
-    base_ptr[r] = (uint64_t)p;
     if (!cl->shared_device)
       for (uint32_t q = 0; q < G; q++)
         if (q != r) {
@@ -2461,15 +2630,7 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     cudaSetDevice(cl->dev[r]);
     cudaDeviceSynchronize();
   }
-  for (uint32_t r = 0; r < G && rc == DINT_OK; r++) {
-    dint_peer_ptrs in[kMaxSets]{}, rb[kMaxSets]{}, sig{};
-    for (uint32_t s = 0; s < S; s++)
-      for (uint32_t o = 0; o < G; o++) { in[s].p[o] = base_ptr[o] + (2 * s) * region; rb[s].p[o] = base_ptr[o] + (2 * s + 1) * region; }
-    for (uint32_t o = 0; o < G; o++) sig.p[o] = base_ptr[o] + 2 * S * region;
-    dint_shard_ctx* c = nullptr;
-    rc = shard_make(cl->eng[r], G, r, cl->cap, S, in, rb, &sig, cl->max_n, cl->shared_device, &c);
-    if (rc == DINT_OK) cl->sh.push_back(c);
-  }
+  if (rc == DINT_OK) rc = cluster_ranks(cl, cl->eng, cl->sh);
   if (rc != DINT_OK) { std::string keep = g_last_error; dint_cluster_destroy(cl); g_last_error = keep; return rc; }
   *out = cl;
   return DINT_OK;
@@ -2478,7 +2639,7 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
 extern "C" {
 
 int dint_cluster_create(int kind, const dint_cfg* cfg, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
-  return cluster_make(kind, cfg, n_gpus, devices, max_batch, nullptr, nullptr, out);
+  return cluster_make(kind, cfg, n_gpus, devices, max_batch, nullptr, nullptr, nullptr, out);
 }
 
 int dint_cluster_image_save(dint_cluster* cl, const char* dir) {
@@ -2510,9 +2671,14 @@ int dint_cluster_image_save(dint_cluster* cl, const char* dir) {
   return rc;
 }
 
-int dint_cluster_image_open(const char* dir, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
+}  // extern "C"
+
+// dint_cluster_image_open; with `rebuilt` dint_cluster_image_open_rebuild
+static int cluster_image_open(const char* dir, int n_gpus, const int* devices, uint64_t max_batch, uint32_t* rebuilt,
+                              dint_cluster** out) {
   if (!dir || !out) return set_err(DINT_EINVAL, "null argument");
   *out = nullptr;
+  if (rebuilt) *rebuilt = 0;
   for (double& t : g_img_times) t = 0;
   const double t0 = img_now();
   const std::string path = img_manifest_path(dir);
@@ -2527,14 +2693,96 @@ int dint_cluster_image_open(const char* dir, int n_gpus, const int* devices, uin
   if (m.version != kImgVersion) return set_errf(DINT_EINVAL, "image %s: format version %u, this build reads %u", path.c_str(), m.version, kImgVersion);
   if (m.kind >= DINT_NUM_KINDS || (m.cfg.flags & ~kCfgKnownFlags)) return set_errf(DINT_EINVAL, "image %s: unknown kind or option flags", path.c_str());
   if ((uint32_t)n_gpus != m.shards) return set_errf(DINT_EINVAL, "image %s: %u shards, not %d", path.c_str(), m.shards, n_gpus);
+  uint32_t missing = 0;
   for (uint32_t r = 0; r < m.shards; r++) {
     struct stat st;
-    if (stat(img_shard_path(dir, r).c_str(), &st) != 0)
-      return set_errf(DINT_EIO, "image %s: %s", img_shard_path(dir, r).c_str(), strerror(errno));
+    if (stat(img_shard_path(dir, r).c_str(), &st) == 0) continue;
+    if (!rebuilt) return set_errf(DINT_EIO, "image %s: %s", img_shard_path(dir, r).c_str(), strerror(errno));
+    missing |= 1u << r;
   }
-  const int rc = cluster_make((int)m.kind, &m.cfg, n_gpus, devices, max_batch, dir, nullptr, out);
+  if (missing && rebuild_check((int)m.kind, m.cfg, m.shards, missing))   // refused before any CUDA call
+    return set_errf(DINT_EIO, "image %s: shard image(s) %s missing and cannot be rebuilt: %s", dir, mask_names(missing).c_str(),
+                    g_last_error.c_str());
+  if (rebuilt) { for (double& t : g_rebuild_times) t = 0; *rebuilt = missing; }
+  const int rc = cluster_make((int)m.kind, &m.cfg, n_gpus, devices, max_batch, dir, nullptr, rebuilt, out);
+  if (rc && rebuilt) *rebuilt = 0;
   g_img_times[0] = img_now() - t0;
+  if (rebuilt) g_rebuild_times[0] = g_img_times[0];
   return rc;
+}
+
+extern "C" {
+
+int dint_cluster_image_open(const char* dir, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
+  return cluster_image_open(dir, n_gpus, devices, max_batch, nullptr, out);
+}
+
+int dint_cluster_image_open_rebuild(const char* dir, int n_gpus, const int* devices, uint64_t max_batch, uint32_t* rebuilt_mask,
+                                    dint_cluster** out) {
+  if (!rebuilt_mask) return set_err(DINT_EINVAL, "null argument");
+  return cluster_image_open(dir, n_gpus, devices, max_batch, rebuilt_mask, out);
+}
+
+int dint_cluster_rebuild(dint_cluster* cl, uint32_t lost_mask) {
+  if (!cl) return set_err(DINT_EINVAL, "null argument");
+  { int rc = rebuild_check(cl->kind, cl->base, cl->G, lost_mask); if (rc) return rc; }
+  if (cl->txn_clients)
+    return set_errf(DINT_EINVAL, "rebuild: %u dint_txn_clients are attached; clients mid-transaction hold locks the rebuilt "
+                                 "shards do not, so destroy them first", cl->txn_clients);
+  for (double& t : g_rebuild_times) t = 0;
+  const double t0 = img_now();
+  for (uint32_t r = 0; r < cl->G; r++) {               // quiesce every device, as dint_cluster_reshard does
+    CU(cudaSetDevice(cl->dev[r]));
+    CU(cudaDeviceSynchronize());
+  }
+  const uint32_t G = cl->G;
+  RebuildFrom f;
+  { int rc = rebuild_prepare(f, cl->eng, G, lost_mask); if (rc) return rc; }
+  g_rebuild_times[2] += img_now() - t0;
+  // the new engines and rank contexts are made next to the old ones, so a failure leaves the cluster as it was
+  std::vector<dint_engine*> eng = cl->eng;
+  std::vector<dint_shard_ctx*> sh;
+  auto fail = [&](int code) {
+    std::string keep = g_last_error;
+    for (auto* c : sh) dint_shard_destroy(c);
+    for (uint32_t r = 0; r < G; r++) {
+      if (eng[r] != cl->eng[r]) dint_destroy(eng[r]);
+      cl->eng[r]->plain_launches = true;               // (dint_shard_destroy cleared it; the old contexts stay)
+    }
+    g_last_error = keep;
+    return code;
+  };
+  for (uint32_t r = 0; r < G; r++)
+    if ((lost_mask >> r) & 1u) {
+      eng[r] = nullptr;
+      int rc = rebuild_engine(f, r, cl->kind, cluster_shard_cfg(cl, r), cl->dev[r], &eng[r]);
+      if (rc) { if (!eng[r]) eng[r] = cl->eng[r]; return fail(rc); }
+    }
+  { int rc = cluster_ranks(cl, eng, sh); if (rc) return fail(rc); }
+  // commit: every rank's epoch restarts at 0 over zeroed signal blocks
+  for (auto* c : cl->sh) dint_shard_destroy(c);
+  for (uint32_t r = 0; r < G; r++) {
+    CU(cudaSetDevice(cl->dev[r]));
+    CU(cudaMemset((void*)cluster_sig_block(cl, r), 0, 4096));
+  }
+  for (uint32_t r = 0; r < G; r++) {
+    if (eng[r] != cl->eng[r]) dint_destroy(cl->eng[r]);
+    eng[r]->plain_launches = true;
+  }
+  cl->eng = eng;
+  cl->sh = sh;
+  for (uint32_t r = 0; r < G; r++) {
+    CU(cudaSetDevice(cl->dev[r]));
+    CU(cudaDeviceSynchronize());
+  }
+  g_rebuild_times[0] = img_now() - t0;
+  return DINT_OK;
+}
+
+int dint_rebuild_times(double out[3]) {
+  if (!out) return set_err(DINT_EINVAL, "null argument");
+  for (int i = 0; i < 3; i++) out[i] = g_rebuild_times[i];
+  return DINT_OK;
 }
 
 int dint_cluster_reshard(dint_cluster* src, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
@@ -2556,7 +2804,7 @@ int dint_cluster_reshard(dint_cluster* src, int n_gpus, const int* devices, uint
   f.src = src;
   { int rc = reshard_count_keys(f, (uint32_t)n_gpus); if (rc) return rc; }
   g_reshard_times[2] += img_now() - t0;
-  const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, out);
+  const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, nullptr, out);
   g_reshard_times[0] = img_now() - t0;
   return rc;
 }
@@ -3010,6 +3258,7 @@ void dint_txn_clients_destroy(dint_txn_clients* t) {
   if (!t->rk.empty()) cudaSetDevice(t->cl->dev[0]);
   if (t->t_beg) cudaEventDestroy(t->t_beg);
   if (t->t_end) cudaEventDestroy(t->t_end);
+  t->cl->txn_clients--;
   delete t;
 }
 
@@ -3022,6 +3271,7 @@ int dint_txn_clients_create(dint_cluster* cl, uint32_t n_clients, uint32_t gid0,
   const uint32_t G = cl->G, msg = kMsgSize[cl->kind];
   dint_txn_clients* t = new dint_txn_clients();
   t->cl = cl; t->msg = msg; t->n = n_clients;
+  cl->txn_clients++;                                   // (dint_txn_clients_destroy counts it down, also on failure below)
   txn::Cfg w{G, subscribers, 0};
   if (cl->kind == DINT_SMALLBANK) {
     w.hot = (uint32_t)((uint64_t)subscribers * 960000 / 24000000);   // kHotAccountNum / kAccountNum, as txn_workloads.cc

@@ -20,6 +20,7 @@
 // the `meta` word, which is claimed with atomicCAS.
 #pragma once
 #include <functional>
+#include <type_traits>
 #include "engine.cuh"
 #ifdef __CUDACC__
 #include <cooperative_groups.h>
@@ -1132,11 +1133,12 @@ __global__ void __launch_bounds__(256) k_kv_load(const Ctx c, int table, const u
   if (!kv_insert_words<VALSZ>(t, key, h, w)) atomicAdd(&c.counters[0], 1ULL);
 }
 
-// Rehash of one table into a fresh (zeroed) array: every FULL entry moves with its version, tombstones vanish.
-// n_owners > 1 (a re-shard, reshard.cuh): only the entries whose global group (fasthash64(key) % to.lock_mod, the
-// reference's bucket) is owned by shard `owner` of n_owners move; `from` may then sit in a peer device's memory.
-template <int VALSZ>
-__global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvTable to, uint32_t n_owners, uint32_t owner) {
+// Every FULL entry of `from` is inserted into `to` with its version; tombstones vanish.  `from` may sit in a peer
+// device's memory, and the caller sizes `to` for every key it receives.  Filters: with n_owners > 1 (a re-shard,
+// reshard.cuh) only the entries whose global group (fasthash64(key) % to.lock_mod, the reference's bucket) is owned by
+// shard `owner` of n_owners; with a Keep (a rebuild, rebuild.cuh) only the entries for which keep(key) holds.
+template <int VALSZ, class Keep = void>
+DINT_D void kv_move_rows(const KvTable& from, const KvTable& to, uint32_t n_owners, uint32_t owner, const Keep* keep = nullptr) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= from.cap_mask; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t* e = from.entries + (i << from.ent_shift);
     uint4 v[Ent<VALSZ>::NV];
@@ -1144,13 +1146,23 @@ __global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvT
     if (v[0].w != ENT_FULL) continue;
     const uint64_t key = ((uint64_t)v[0].y << 32) | v[0].x;
     const uint64_t h = fasthash64_u64(key);
-    if (n_owners > 1 && fast_mod(h, to.lock_mod) % n_owners != owner) continue;
+    if constexpr (std::is_void_v<Keep>) {
+      if (n_owners > 1 && fast_mod(h, to.lock_mod) % n_owners != owner) continue;
+    } else {
+      if (!(*keep)(key)) continue;
+    }
     uint32_t w[Ent<VALSZ>::NW];
     const uint32_t* flat = (const uint32_t*)v;
 #pragma unroll
     for (int k = 0; k < Ent<VALSZ>::NW; k++) w[k] = flat[4 + k];
     kv_insert_words<VALSZ>(to, key, h, w, v[0].z);   // (`to` has room for every key it receives: cannot fail)
   }
+}
+
+// Rehash of one table into a fresh (zeroed) array, or (n_owners > 1) one source table's share of a re-shard.
+template <int VALSZ>
+__global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvTable to, uint32_t n_owners, uint32_t owner) {
+  kv_move_rows<VALSZ>(from, to, n_owners, owner);
 }
 
 // valid slots of table `table`'s chain entries (dint_kv_count with the eBPF tier): freed entries hold none
@@ -1251,6 +1263,12 @@ inline int kv_plan(int kind, const dint_cfg& cf, bool tatp_ebpf, KvPlan& p) {
   }
   return DINT_OK;
 }
+// log2 capacity of a table filled with `keys` keys at once (re-shard, rebuild): at least lg, and large enough that the
+// keys load it to <= 35 %, so kv_maintain does not rehash it on the next call; > 34 = too many keys
+inline uint32_t kv_fit_log2(uint32_t lg, uint64_t keys) {
+  while (lg <= 34 && keys * 20 > (7ULL << lg)) lg++;
+  return lg;
+}
 
 template <typename AllocFn>
 int kv_create_tables(int kind, const dint_cfg& cf, Ctx& c, KvHost* kv, uint64_t* groups_out, AllocFn alloc, bool tatp_ebpf = false) {
@@ -1350,6 +1368,21 @@ inline int tatp_select_types(uint64_t* seed, uint8_t out[4]) {   // tatp/udp/tat
   return got;
 }
 
+// ---- tatp / smallbank replica placement (txn_clients.cuh: primary p = key % G, backups (p + 1) % G and (p + 2) % G) -----
+// G is the placement's shard count: dint_cfg.txn_shards > 3 ? txn_shards : 3 for one engine (with three shards or fewer
+// every shard holds every key), the shard count for a cluster.  p = key % G.
+// The role of `shard` for the keys of residue p: 0 primary, 1 or 2 backup, > 2 not one of their replicas.
+DINT_HD uint32_t txn_role(uint32_t p, uint32_t G, uint32_t shard) { return (shard + G - p) % G; }
+// The shard a rebuild copies the rows of residue p from when the shards of bit mask `lost` are lost: the surviving
+// replica with the lowest role, or -1 when every replica is lost (dint_cluster_rebuild).
+DINT_HD int rebuild_source(uint32_t p, uint32_t G, uint32_t lost) {
+  for (uint32_t i = 0; i < 3; i++) {
+    const uint32_t s = (p + i) % G;                  // the shard of role i: txn_role(p, G, s) == i
+    if (!((lost >> s) & 1u)) return (int)s;
+  }
+  return -1;
+}
+
 struct KvBatch {
   std::vector<uint64_t> keys;
   std::vector<uint8_t> vals;
@@ -1365,9 +1398,9 @@ struct KvBatch {
   uint32_t G = 0, gid = 0;                           // replica filter (dint_cfg.txn_shards / txn_shard_id)
   std::vector<uint8_t> dummy;
   uint8_t* add(uint64_t key) {                       // returns the zeroed value slot
-    if (G > 3) {                                     // not one of this key's three replica holders: drop it
-      const uint32_t p = (uint32_t)(key % G), d = (gid + G - p) % G;
-      if (d > 2) { dummy.assign(valsz, 0); return dummy.data(); }
+    if (G > 3 && txn_role((uint32_t)(key % G), G, gid) > 2) {   // not one of this key's three replica holders: drop it
+      dummy.assign(valsz, 0);
+      return dummy.data();
     }
     if (keys.size() == (1u << 20)) flush();
     keys.push_back(key);

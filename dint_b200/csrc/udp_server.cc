@@ -31,7 +31,8 @@
 // usage: dint_udp_server <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind A.B.C.D]
 //                        [--sockets R] [--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shard-id I --shards G]
 //                        [--linger-us U] [--populate N] [--mon-port 20231] [--lock-holder-keys]
-//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH] [--image-out PATH]
+//                        [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH [--rebuild-lost]]
+//                        [--image-out PATH]
 //
 // --lock-holder-keys (tatp): DINT_CFG_LOCK_HOLDER_KEYS -- a refused kAcquireLock is answered kRejectLockSameKey (28) when
 // the lock is held for the same key and kRejectLock (8) when another key shares the slot, as the reference's eBPF lock
@@ -56,7 +57,9 @@
 // --image-in PATH: start from a state image (include/dint_b200.h, "State images") instead of populating: a file written by
 // dint_image_save, or with --gpus G > 1 a directory written by dint_cluster_image_save.  Its kind and option flags must
 // be the command line's, and for tatp / smallbank with --shards G --shard-id I it must be shard I of G, else the server
-// exits with 2.  --image-out PATH: on SIGINT / SIGTERM, once the engine threads
+// exits with 2.  --rebuild-lost (tatp / smallbank with --gpus G > 1): a shard image of the --image-in directory that is
+// missing, short or corrupt is rebuilt from the other shards' replicas (dint_cluster_image_open_rebuild) and the server
+// names the shards it rebuilt; without it such a directory stops start-up.  --image-out PATH: on SIGINT / SIGTERM, once the engine threads
 // have stopped and the last replies are sent, write the state to PATH (the same file / directory forms); the exit code
 // is 1 if that fails.
 //
@@ -95,6 +98,7 @@ extern "C" {
 #pragma weak dint_image_save
 #pragma weak dint_cluster_image_open
 #pragma weak dint_cluster_image_save
+#pragma weak dint_cluster_image_open_rebuild
 
 namespace {
 
@@ -141,7 +145,7 @@ int open_socket(const sockaddr_in& addr, bool reuseport) {
 int main(int argc, char** argv) {
   if (argc < 2) {
     fprintf(stderr, "usage: %s <lock_2pl|lock_fasst|log_server|store|tatp|smallbank> [--port P] [--bind ADDR] [--sockets R] "
-                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH] [--image-out PATH]\n", argv[0]);
+                    "[--batch N] [--device D] [--gpus G [--devices a,b,..]] [--shards G --shard-id I] [--linger-us U] [--populate N] [--lock-holder-keys] [--store-ebpf wb-bloom|wb|wt] [--tatp-ebpf] [--smallbank-ebpf] [--image-in PATH [--rebuild-lost]] [--image-out PATH]\n", argv[0]);
     return 2;
   }
   const int kind = kind_of(argv[1]);
@@ -153,13 +157,14 @@ int main(int argc, char** argv) {
   if (n_sock > 8) n_sock = 8;                         // the reference runs `server 8` (exp/run_lock_fasst.sh)
   std::string bind_addr = "0.0.0.0", image_in, image_out;
   std::vector<int> devices;
-  bool holder_keys = false, tatp_ebpf = false, smallbank_ebpf = false;
+  bool holder_keys = false, tatp_ebpf = false, smallbank_ebpf = false, rebuild_lost = false;
   uint32_t store_ebpf = 0;
   for (int i = 2; i < argc; i += 2) {
     const std::string a = argv[i];
     if (a == "--lock-holder-keys") { holder_keys = true; i--; continue; }   // the three options without a value
     if (a == "--tatp-ebpf") { tatp_ebpf = true; i--; continue; }
     if (a == "--smallbank-ebpf") { smallbank_ebpf = true; i--; continue; }
+    if (a == "--rebuild-lost") { rebuild_lost = true; i--; continue; }
     if (i + 1 >= argc) break;
     const char* v = argv[i + 1];
     if (a == "--port") port = atoi(v);
@@ -194,11 +199,19 @@ int main(int argc, char** argv) {
     fprintf(stderr, "dint_udp_server: this libdint_b200.so has no state images (--image-in / --image-out)\n");
     return 1;
   }
+  const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
+  if (rebuild_lost && (image_in.empty() || gpus < 2 || !by_dst)) {
+    fprintf(stderr, "--rebuild-lost needs --image-in DIR with --gpus G > 1 and a tatp or smallbank server\n");
+    return 2;
+  }
+  if (rebuild_lost && !dint_cluster_image_open_rebuild) {
+    fprintf(stderr, "dint_udp_server: this libdint_b200.so cannot rebuild shards (--rebuild-lost)\n");
+    return 1;
+  }
   sockaddr_in srv{};
   srv.sin_family = AF_INET;
   if (inet_pton(AF_INET, bind_addr.c_str(), &srv.sin_addr) != 1) { fprintf(stderr, "bad --bind address\n"); return 2; }
   const uint32_t msg = dint_msg_size(kind);
-  const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
   const int n_groups = (gpus > 1 && by_dst) ? gpus : 1;        // one well-known port per shard server
 
   // ---- engine: the state the reference keeps in its global arrays lives on the GPU(s) ----
@@ -236,11 +249,20 @@ int main(int argc, char** argv) {
               img_cfg.txn_shard_id, placement(img_cfg.txn_shards), shard_id, placement(shards));
       return 2;
     }
-    const int rc = dir ? dint_cluster_image_open(image_in.c_str(), gpus, devices.empty() ? nullptr : devices.data(), 0, &cluster)
-                       : dint_image_open(image_in.c_str(), device, &eng);
+    uint32_t rebuilt = 0;
+    const int* dv = devices.empty() ? nullptr : devices.data();
+    const int rc = rebuild_lost ? dint_cluster_image_open_rebuild(image_in.c_str(), gpus, dv, 0, &rebuilt, &cluster)
+                   : dir        ? dint_cluster_image_open(image_in.c_str(), gpus, dv, 0, &cluster)
+                                : dint_image_open(image_in.c_str(), device, &eng);
     if (rc != DINT_OK) {
       fprintf(stderr, "dint_udp_server: opening the image failed: %s\n", dint_last_error());
       return 1;
+    }
+    if (rebuild_lost) {
+      std::string names;
+      for (int r = 0; r < gpus; r++)
+        if ((rebuilt >> r) & 1u) names += (names.empty() ? "" : ", ") + std::to_string(r);
+      fprintf(stderr, "dint_udp_server: rebuilt shard(s) {%s} of %s from their replicas\n", names.c_str(), image_in.c_str());
     }
   } else if (gpus > 1) {
     if (dint_cluster_create(kind, &cfg, gpus, devices.empty() ? nullptr : devices.data(), 0, &cluster) != DINT_OK ||

@@ -76,10 +76,10 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_cluster_reshard", "dint_reshard_times", "dint_cluster_clients_rebind", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_cluster_reshard", "dint_reshard_times", "dint_cluster_rebuild", "dint_cluster_image_open_rebuild", "dint_rebuild_times", "dint_cluster_clients_rebind", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
-    "dint_test_fasthash64", "dint_test_fastmod", "dint_test_host_slices",
+    "dint_test_fasthash64", "dint_test_fastmod", "dint_test_rebuild_source", "dint_test_host_slices",
 ]
 
 
@@ -152,6 +152,10 @@ def lib():
     L.dint_image_times.restype = i32; L.dint_image_times.argtypes = [C.POINTER(C.c_double)]
     L.dint_cluster_reshard.restype = i32; L.dint_cluster_reshard.argtypes = [vp, i32, C.POINTER(i32), u64, C.POINTER(vp)]
     L.dint_reshard_times.restype = i32; L.dint_reshard_times.argtypes = [C.POINTER(C.c_double)]
+    L.dint_cluster_rebuild.restype = i32; L.dint_cluster_rebuild.argtypes = [vp, u32]
+    L.dint_cluster_image_open_rebuild.restype = i32
+    L.dint_cluster_image_open_rebuild.argtypes = [C.c_char_p, i32, C.POINTER(i32), u64, C.POINTER(u32), C.POINTER(vp)]
+    L.dint_rebuild_times.restype = i32; L.dint_rebuild_times.argtypes = [C.POINTER(C.c_double)]
     L.dint_cluster_clients_rebind.restype = i32; L.dint_cluster_clients_rebind.argtypes = [vp, vp]
     L.dint_shard_destroy.restype = None; L.dint_shard_destroy.argtypes = [vp]
     L.dint_shard_submit_many.restype = i32; L.dint_shard_submit_many.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(vp), u64, C.POINTER(vp), vp]
@@ -181,6 +185,7 @@ def lib():
     L.dint_host_free.restype = None; L.dint_host_free.argtypes = [vp]
     L.dint_test_fasthash64.restype = u64; L.dint_test_fasthash64.argtypes = [u64, i32]
     L.dint_test_fastmod.restype = u32; L.dint_test_fastmod.argtypes = [u64, u32]
+    L.dint_test_rebuild_source.restype = i32; L.dint_test_rebuild_source.argtypes = [u64, u32, u32]
     _lib = L
     return L
 
@@ -245,6 +250,14 @@ def reshard_times():
     allocation of the destination (dint_reshard_times)."""
     out = (C.c_double * 3)()
     lib().dint_reshard_times(out)
+    return {"wall_s": out[0], "kernel_s": out[1], "count_alloc_s": out[2]}
+
+
+def rebuild_times():
+    """Seconds spent by this thread's last rebuild (GpuCluster.rebuild, or GpuCluster.open_image with rebuild=True): wall,
+    rebuild kernels (CUDA events), row count + allocation of the new engines (dint_rebuild_times)."""
+    out = (C.c_double * 3)()
+    lib().dint_rebuild_times(out)
     return {"wall_s": out[0], "kernel_s": out[1], "count_alloc_s": out[2]}
 
 
@@ -705,9 +718,14 @@ class GpuCluster:
             raise DintError(rc, f"dint_cluster_image_save({path})")
 
     @classmethod
-    def open_image(cls, path, devices=None, max_batch=0):
+    def open_image(cls, path, devices=None, max_batch=0, rebuild=False):
         """A new cluster holding the state saved in directory `path` (dint_cluster_image_open); one shard per entry of
-        `devices` (default: as many shards as were saved, on devices 0..G-1)."""
+        `devices` (default: as many shards as were saved, on devices 0..G-1).  rebuild=True (tatp / smallbank,
+        dint_cluster_image_open_rebuild): a shard image that is missing, short or corrupt is rebuilt from the other
+        shards' replicas, and `.rebuilt` lists the shards rebuilt.  To repair a directory, save the result to ANOTHER
+        one: a save removes the manifest before it rewrites shards."""
+        if not isinstance(rebuild, bool):
+            raise TypeError("rebuild must be True or False")
         if devices is not None:
             n = len(devices)
         else:                                   # as many shards as were saved; an unreadable manifest is the C call's to refuse
@@ -717,13 +735,36 @@ class GpuCluster:
                 n = 0
         dv = (C.c_int * n)(*devices) if devices is not None else None
         h = C.c_void_p()
-        rc = lib().dint_cluster_image_open(os.fsencode(path), n, dv, max_batch, C.byref(h))
+        mask = C.c_uint32(0)
+        if rebuild:
+            rc = lib().dint_cluster_image_open_rebuild(os.fsencode(path), n, dv, max_batch, C.byref(mask), C.byref(h))
+        else:
+            rc = lib().dint_cluster_image_open(os.fsencode(path), n, dv, max_batch, C.byref(h))
         if rc != 0:
-            raise DintError(rc, f"dint_cluster_image_open({path})")
+            raise DintError(rc, f"dint_cluster_image_open{'_rebuild' if rebuild else ''}({path})")
         hdr = read_image_header(path)
         cl = cls.__new__(cls)
         cl.kind, cl.msg, cl.G, cl.cfg, cl.h = hdr["kind"], MSG_SIZE[hdr["kind"]], n, hdr["cfg"], h
+        if rebuild:
+            cl.rebuilt = [r for r in range(n) if (mask.value >> r) & 1]
         return cl
+
+    def rebuild(self, shards):
+        """Rebuild the listed shards of this tatp / smallbank cluster in place from the surviving replicas
+        (dint_cluster_rebuild): each gets a new engine holding, for every key it replicates, the row of the key's
+        surviving replica with the lowest role; lock state, the log ring and statistics start empty.  No GPU
+        transaction clients may be attached.  On failure the cluster is unchanged."""
+        if isinstance(shards, (int, np.integer)):
+            raise TypeError("shards: a list of shard indices")
+        shards = list(shards)
+        if not shards or any(isinstance(s, bool) or not isinstance(s, (int, np.integer)) for s in shards):
+            raise ValueError(f"shards: a non-empty list of shard indices, not {shards!r}")
+        if len(set(shards)) != len(shards) or any(not 0 <= s < self.G for s in shards):
+            raise ValueError(f"shards {shards}: distinct indices in [0, {self.G}) expected")
+        mask = sum(1 << int(s) for s in shards)
+        rc = lib().dint_cluster_rebuild(self.h, mask)
+        if rc != 0:
+            raise DintError(rc, f"dint_cluster_rebuild({KIND_NAMES[self.kind]}, shards {sorted(shards)})")
 
     def reshard(self, n_shards, devices=None, max_batch=0):
         """A new cluster of `n_shards` shards holding this one's state (dint_cluster_reshard): it answers every later

@@ -505,6 +505,56 @@ int dint_cluster_reshard(dint_cluster *src, int n_gpus, const int *devices, uint
 int dint_reshard_times(double out[3]);
 
 /*
+ * Rebuilding lost tatp / smallbank shards from their replicas.
+ *   Placement: the engine's own.  A cluster of G shards (G = 1 or 3..8; an engine alone places with
+ *     txn_shards > 3 ? txn_shards : 3) keeps the rows of key k on its three replicas, shards (k % G + i) % G of roles
+ *     i = 0 (primary), 1 and 2 (backups): the clients write every row there (txn_clients.cuh), and population places
+ *     rows the same way, so each shard holds every row of every key it is a replica of.  With G = 3 every shard holds
+ *     every key.
+ *   Lost set: any set of shards that leaves every key at least one surviving replica -- for G >= 4 no three cyclically
+ *     consecutive shards, for G = 3 at most two.  G = 1 has nothing to rebuild from.
+ *   Source rule: for each key the source is its surviving replica with the lowest role; that copy (value and version) is
+ *     inserted once into every lost replica of the key.  The rule depends on (k, G, lost set) alone, so the result is
+ *     deterministic.
+ *   Exactness: at a replica-consistent point -- every write served at all of its replicas: after population, or after
+ *     traffic made of whole transactions -- a rebuilt shard's rows equal the lost shard's: the same keys in every table,
+ *     the same values and versions (kCommitBck bumps a version exactly as kCommitPrim does), and deleted rows absent.
+ *   Mid-transaction: the clients commit the log, then the backups, then the primary, in separate rounds.  At a round
+ *     boundary the backups can be one write ahead of a primary that still holds that key's lock, and a rebuilt primary
+ *     then takes the backups' newer row.
+ *   Not rebuilt, because it cannot be: TATP lock words and holder keys, and SmallBank's {num_ex, num_sh} counters, start
+ *     free (a lock slot is shared by keys of different primaries, so a peer's slot cannot be attributed to keys); the
+ *     log ring starts empty (for G > 3 a shard's arrival order cannot be recovered from its peers, and nothing reads
+ *     the log); statistics start at zero, as after an image open.
+ *   dint_cluster_rebuild: rebuild the shards of bit mask lost_mask in place.  It synchronises every device (a quiesce
+ *     point, as dint_cluster_reshard), builds each lost shard's new engine on that shard's device from the shard's
+ *     configuration (its tables at least as large as dint_cluster_create makes them, and large enough to keep their
+ *     rows at <= 35 % load) and fills it from the surviving replicas over peer memory; the old engine's state is never
+ *     read.  Only then the new engines replace the old ones, and every rank's exchange context is made again over the
+ *     cluster's exchange buffers, signal blocks zeroed, as dint_cluster_create makes them.  On any failure the cluster is
+ *     left as it was.  Peak device memory: the cluster plus the new engines.
+ *     DINT_EINVAL, the cluster unchanged: lock_2pl, lock_fasst, store and log_server clusters (no replicas); G = 1; an
+ *     empty mask or one naming shards outside [0, G); a lost set that leaves some key without a replica;
+ *     DINT_CFG_TATP_EBPF and DINT_CFG_SMALLBANK_EBPF (their cache tiers hold dirty and cache-only rows whose wire-visible
+ *     versions depend on each shard's own hit history); and a cluster with dint_txn_clients attached (clients
+ *     mid-transaction hold locks that are lost -- a SmallBank release would drive a counter below zero).
+ *   dint_cluster_image_open_rebuild: dint_cluster_image_open, except that a shard image that is missing or fails with
+ *     DINT_EIO (short file, I/O error, checksum) is rebuilt from the others, which are opened first.  *rebuilt_mask
+ *     receives the shards rebuilt (0: the image was whole).  The manifest must be valid (DINT_EIO when missing), and
+ *     DINT_EINVAL from a shard image (foreign kind, flags, layout) stays an error.  A failed set that cannot be rebuilt
+ *     (by the rules above) returns DINT_EIO naming the shards; missing files are judged before any CUDA call.  The shard
+ *     images of one directory are of one moment (the manifest is written last), so the rebuilt rows are those the lost
+ *     shard saved.  To repair a directory, open it this way and save to ANOTHER directory: a save removes the manifest
+ *     before it rewrites shards, so an in-place repair that stopped part-way would leave nothing to open.
+ *   dint_rebuild_times: the last rebuild of this thread, in seconds: [0] wall, [1] the rebuild kernels (CUDA events,
+ *     summed over the lost shards), [2] the row count and the new engines' allocation.
+ */
+int dint_cluster_rebuild(dint_cluster *c, uint32_t lost_mask);
+int dint_cluster_image_open_rebuild(const char *dir, int n_gpus, const int *devices, uint64_t max_batch, uint32_t *rebuilt_mask,
+                                    dint_cluster **out);
+int dint_rebuild_times(double out[3]);
+
+/*
  * lock_2pl, lock_fasst, log_server and store closed-loop clients ON the GPU (SURVEY.md section 8(f) rank 2).  The
  * reference's clients are Caladan uthreads on other machines (lock_2pl/caladan/client.cc:181-230,
  * lock_fasst/caladan/client.cc:183-280, store/caladan/client_udp.cc:135-208; trace shapes lock_2pl/caladan/
@@ -632,6 +682,9 @@ void dint_host_free(void *p);
 /* hooks for unit tests of the host/device-shared arithmetic (no GPU needed) */
 uint64_t dint_test_fasthash64(uint64_t x, int len);      /* len 4 or 8, seed 0xdeadbeef */
 uint32_t dint_test_fastmod(uint64_t n, uint32_t d);
+/* the source shard dint_cluster_rebuild copies key's rows from in a G-shard cluster that lost the shards of lost_mask,
+ * or -1 when every replica of the key is lost (or G is outside 1..8) */
+int dint_test_rebuild_source(uint64_t key, uint32_t G, uint32_t lost_mask);
 /* test hook: the slice sizes dint_submit cuts a call of n requests into (host logic, no GPU needed);
  * returns the number of slices, writes the first `cap` of them */
 uint32_t dint_test_host_slices(uint64_t n, uint32_t min_slice, uint32_t max_slice, int ramp_up, uint32_t *out, uint32_t cap);
