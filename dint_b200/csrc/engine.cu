@@ -403,7 +403,7 @@ static int kv_maintain(dint_engine* e, cudaStream_t s) {
       ProfScope ps(e, s, KT_LOAD);
       with_kind(exec_kind(e), [&](auto k) {
         constexpr int K = decltype(k)::value;
-        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK || K == K_SMALLBANK_EBPF) k_kv_rehash<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N, 1u, 0u);
+        if constexpr (K == K_STORE || K == K_STORE_EBPF || K == K_TATP || K == K_SMALLBANK || K == K_SMALLBANK_EBPF) k_kv_move<Wire<K>::VALSZ><<<e->sms * 8, 256, 0, s>>>(T, N, KeepAll{});
         return DINT_OK;
       });
     }
@@ -421,6 +421,21 @@ static int kv_publish_counts(dint_engine* e, cudaStream_t s) {
   if (e->ctx.n_tables == 0 || !e->h_kvcnt) return DINT_OK;
   CU(cudaMemcpyAsync(e->h_kvcnt, e->ctx.tbl[0].live, 16 * e->ctx.n_tables, cudaMemcpyDeviceToHost, s));   // (the tables' counters are contiguous)
   CU(cudaEventRecord(e->ev_kvcnt, s));
+  return DINT_OK;
+}
+
+// an engine being made from state held elsewhere (an image, a re-shard, a rebuild): destroyed unless released
+struct EngineOwner {
+  dint_engine* e;
+  ~EngineOwner() { if (e) dint_destroy(e); }
+};
+// The last step of making such an engine.  Its KV tables' {live, used} counters were written with the state: set up
+// and refresh their host mirror, as dint_snapshot_restore does, so that the next call's kv_maintain decides on them.
+static int engine_ready(dint_engine* e) {
+  { int rc = kv_maintain(e, e->stream); if (rc) return rc; }
+  { int rc = kv_publish_counts(e, e->stream); if (rc) return rc; }
+  CU(cudaStreamSynchronize(e->stream));
+  e->stats = dint_stats{};
   return DINT_OK;
 }
 
@@ -1385,7 +1400,7 @@ static int image_open_impl(const char* path, int device, const dint_cfg* want, d
   }
   dint_engine* e = nullptr;
   { int rc = dint_create((int)h.kind, &cfg, device, &e); if (rc) return rc; }
-  struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
+  EngineOwner own{e};
   std::vector<std::pair<void*, size_t>> regs;
   snapshot_regions(e, regs);
   if (regs.size() != h.n_regions || e->ctx.tpool_cap != h.tpool_cap)
@@ -1451,12 +1466,7 @@ static int image_open_impl(const char* path, int device, const dint_cfg* want, d
   if (N) CU(cudaMemcpy(bad.data(), P.bad, 4 * N, cudaMemcpyDeviceToHost));
   for (uint64_t j = 0; j < N; j++)
     if (bad[j]) return set_errf(DINT_EIO, "image %s: region %u block %llu: checksum mismatch", path, blocks[j].region, (unsigned long long)blocks[j].index);
-  // the KV tables' {live, used} counters came back too: set up and refresh their host mirror, as dint_snapshot_restore
-  // does, so that the next call's kv_maintain decides on the saved occupancy
-  { int rc = kv_maintain(e, e->stream); if (rc) return rc; }
-  { int rc = kv_publish_counts(e, e->stream); if (rc) return rc; }
-  CU(cudaStreamSynchronize(e->stream));
-  e->stats = dint_stats{};
+  { int rc = engine_ready(e); if (rc) return rc; }
   own.e = nullptr;
   *out = e;
   return DINT_OK;
@@ -2323,12 +2333,9 @@ void dint_cluster_destroy(dint_cluster* cl) {
 
 }  // extern "C"
 
-// ---- re-sharding (dint_cluster_reshard; reshard.cuh has the ownership arithmetic) ----------------------------------
+// ---- shards derived from other shards' state (dint_cluster_reshard, dint_cluster_rebuild) ---------------------------
 static thread_local double g_reshard_times[3];       // dint_reshard_times: wall, re-shard kernels, count + allocation (s)
-struct ReshardFrom {
-  const dint_cluster* src = nullptr;
-  std::vector<uint64_t> keys;                        // store: the live keys each destination shard receives
-};
+static thread_local double g_rebuild_times[3];       // dint_rebuild_times: wall, rebuild kernels, count + allocation (s)
 
 // lets `device` (the current device) read `peer`'s memory; nothing to do when they are the same
 static int peer_enable(int device, int peer) {
@@ -2342,99 +2349,124 @@ static int peer_enable(int device, int peer) {
   return DINT_OK;
 }
 
-// counts, per destination shard of G2, the live keys of every source table (one small copy per source shard)
-static int reshard_count_keys(ReshardFrom& f, uint32_t G2) {
-  const dint_cluster* src = f.src;
-  f.keys.assign(G2, 0);
-  if (src->kind != DINT_STORE) return DINT_OK;
-  for (uint32_t r = 0; r < src->G; r++) {
-    const dint_engine* e = src->eng[r];
-    CU(cudaSetDevice(e->device));
-    unsigned long long* d = nullptr;
-    unsigned long long h[kMaxShards] = {0};
-    CU(cudaMalloc(&d, sizeof h));
-    cudaError_t ce = cudaMemset(d, 0, sizeof h);
-    if (ce == cudaSuccess) {
-      k_kv_owner_count<<<e->sms * 4, kThreads>>>(e->ctx.tbl[0], G2, d);
-      ce = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(d);
-    if (ce != cudaSuccess) return set_err(DINT_EIO, "re-shard key count", ce);
-    for (uint32_t j = 0; j < G2; j++) f.keys[j] += h[j];
+// waits for every device of cl
+static int cluster_quiesce(const dint_cluster* cl) {
+  for (uint32_t r = 0; r < cl->G; r++) {
+    CU(cudaSetDevice(cl->dev[r]));
+    CU(cudaDeviceSynchronize());
   }
   return DINT_OK;
 }
 
-// Destination shard j of G2 on `device`, with configuration c: created as dint_create would (a store table at least
-// large enough to keep the keys it receives at <= 35 % load, so kv_maintain leaves it as it is), then filled from the
-// source shards by the kernels of reshard.cuh on its own stream.
-static int reshard_engine(const ReshardFrom& f, uint32_t j, uint32_t G2, dint_cfg c, int device, dint_engine** out) {
-  const dint_cluster* src = f.src;
+// the shards a re-shard or rebuild reads
+struct DeriveFrom {
+  std::vector<dint_engine*> src;                    // per source shard: its engine (nullptr where a rebuild lost it)
+  uint64_t rows[kMaxShards][kMaxTables] = {};        // the rows each destination shard receives, per table (count_rows)
+};
+
+// f.rows[d][t] += the FULL rows of table t of each engine of `read` (nullptr: not read) that go to destination shard d;
+// dests_of(s, table) is k_kv_count_rows's filter for source s.  One small copy per source.
+template <class DestsOf>
+static int count_rows(DeriveFrom& f, const std::vector<dint_engine*>& read, DestsOf dests_of, const char* what) {
+  for (uint32_t s = 0; s < read.size(); s++) {
+    const dint_engine* e = read[s];
+    if (!e || e->ctx.n_tables == 0) continue;
+    CU(cudaSetDevice(e->device));
+    unsigned long long* d = nullptr;
+    unsigned long long h[kMaxTables][kMaxShards] = {};
+    CU(cudaMalloc(&d, sizeof h));
+    cudaError_t ce = cudaMemset(d, 0, sizeof h);
+    for (uint32_t t = 0; t < e->ctx.n_tables && ce == cudaSuccess; t++) {
+      k_kv_count_rows<<<e->sms * 4, kThreads>>>(e->ctx.tbl[t], dests_of(s, e->ctx.tbl[t]), d + t * kMaxShards);
+      ce = cudaGetLastError();
+    }
+    if (ce == cudaSuccess) ce = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    if (ce != cudaSuccess) return set_err(DINT_EIO, what, ce);
+    for (uint32_t t = 0; t < kMaxTables; t++)
+      for (uint32_t j = 0; j < kMaxShards; j++) f.rows[j][t] += h[t][j];
+  }
+  return DINT_OK;
+}
+
+// Shard j of a derived cluster, of `kind` on `device` with configuration c: created as dint_create would, with every KV
+// table at least large enough to keep the rows[t] it receives at <= 35 % load (so kv_maintain leaves it as it is),
+// given peer access to the engines of `read` (nullptr: not read), filled by fill(e) on its own stream, and made ready.
+// What the fill does not write (a rebuild's lock words, holder keys and log ring) is that of a new engine.
+// times[1] += the fill's CUDA-event time; times[2] += the sizing, allocation and peer set-up.
+template <class Fill>
+static int derive_engine(int kind, dint_cfg c, int device, uint32_t j, const uint64_t* rows, const std::vector<dint_engine*>& read,
+                         double* times, Fill fill, dint_engine** out) {
   *out = nullptr;
-  double t0 = img_now();
-  if (src->kind == DINT_STORE) {
+  const double t0 = img_now();
+  if (kind == DINT_STORE || kind == DINT_TATP || kind == DINT_SMALLBANK) {
     KvPlan P;
-    if (kv_plan(DINT_STORE, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
-    const uint32_t lg = kv_fit_log2(P.lg[0], f.keys[j]);
-    if (lg > 34) return set_errf(DINT_EINVAL, "re-shard: shard %u would receive %llu keys", j, (unsigned long long)f.keys[j]);
-    c.kv_capacity_log2[0] = lg;
+    if (kv_plan(kind, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
+    for (uint32_t t = 0; t < P.nt; t++) {
+      const uint32_t lg = kv_fit_log2(P.lg[t], rows[t]);
+      if (lg > 34)                                     // (a store is re-sharded; tatp and smallbank are rebuilt)
+        return kind == DINT_STORE ? set_errf(DINT_EINVAL, "re-shard: shard %u would receive %llu keys", j, (unsigned long long)rows[t])
+                                  : set_errf(DINT_EINVAL, "rebuild: shard %u table %u would receive %llu rows", j, t, (unsigned long long)rows[t]);
+      c.kv_capacity_log2[t] = lg;
+    }
   }
   dint_engine* e = nullptr;
-  { int rc = dint_create(src->kind, &c, device, &e); if (rc) return rc; }
-  struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
-  for (uint32_t r = 0; r < src->G; r++) {             // the kernels read the source shards' arrays where they are
-    int rc = peer_enable(device, src->dev[r]);
-    if (rc) return rc;
-  }
-  g_reshard_times[2] += img_now() - t0;
-  const Ctx& d = e->ctx;
-  const cudaStream_t s = e->stream;
-  ReshardArgs a{};
-  a.G = src->G; a.G2 = G2; a.j = j; a.src_div = make_fastmod(src->G);
-  a.n_local = (uint32_t)e->total_groups;
-  a.n_global = e->kind == DINT_STORE ? e->kv[0].hash_size : e->cfg.lock_slots;
+  { int rc = dint_create(kind, &c, device, &e); if (rc) return rc; }
+  EngineOwner own{e};
+  for (const dint_engine* s : read)                    // the fill reads the sources' arrays where they are
+    if (s) { int rc = peer_enable(device, s->device); if (rc) return rc; }
+  times[2] += img_now() - t0;
   cudaEvent_t ev[2] = {nullptr, nullptr};
   struct Events { cudaEvent_t* ev; ~Events() { for (int i = 0; i < 2; i++) if (ev[i]) cudaEventDestroy(ev[i]); } } evs{ev};
   for (cudaEvent_t& x : ev) CU(cudaEventCreate(&x));
-  CU(cudaEventRecord(ev[0], s));
-  const int grid = e->sms * 4;
-  if (e->kind == DINT_LOCK2PL) {
-    for (uint32_t r = 0; r < src->G; r++) a.src[r] = (uint64_t)src->eng[r]->ctx.cnt2;
-    a.dst = d.cnt2;
-    k_reshard_lock<K_LOCK2PL><<<grid, kThreads, 0, s>>>(a);
-  } else if (e->kind == DINT_FASST) {
-    for (uint32_t r = 0; r < src->G; r++) { a.src[r] = (uint64_t)src->eng[r]->ctx.ver; a.src_bits[r] = (uint64_t)src->eng[r]->ctx.lockbits; }
-    a.dst = d.ver;
-    a.dst_bits = d.lockbits;
-    k_reshard_lock<K_FASST><<<grid, kThreads, 0, s>>>(a);
-  } else {
-    for (uint32_t r = 0; r < src->G; r++) k_kv_rehash<40><<<e->sms * 8, 256, 0, s>>>(src->eng[r]->ctx.tbl[0], d.tbl[0], G2, j);
-    if (d.ecache) {                                    // the eBPF tier: its sets move whole; its counters start at zero
-      for (uint32_t r = 0; r < src->G; r++) a.src[r] = (uint64_t)src->eng[r]->ctx.ecache;
-      a.dst = d.ecache;
-      k_reshard_sets<<<grid, kThreads, 0, s>>>(a);
-    }
-  }
+  CU(cudaEventRecord(ev[0], e->stream));
+  fill(e);
   CU(cudaGetLastError());
-  CU(cudaEventRecord(ev[1], s));
+  CU(cudaEventRecord(ev[1], e->stream));
   CU(cudaEventSynchronize(ev[1]));
   float ms = 0;
   CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-  g_reshard_times[1] += ms * 1e-3;
-  // the tables' {live, used} counters were recounted by the inserts: set up and refresh their host mirror, as
-  // dint_image_open does, so that the next call's kv_maintain decides on them
-  { int rc = kv_maintain(e, s); if (rc) return rc; }
-  { int rc = kv_publish_counts(e, s); if (rc) return rc; }
-  CU(cudaStreamSynchronize(s));
-  e->stats = dint_stats{};
+  times[1] += ms * 1e-3;
+  { int rc = engine_ready(e); if (rc) return rc; }
   own.e = nullptr;
   *out = e;
   return DINT_OK;
 }
 
-// ---- rebuilding lost tatp / smallbank shards (dint_cluster_rebuild; rebuild.cuh has the placement arithmetic) -----
-static thread_local double g_rebuild_times[3];       // dint_rebuild_times: wall, rebuild kernels, count + allocation (s)
+// Destination shard j of G2, filled from every source shard by the kernels of reshard.cuh (which has the ownership
+// arithmetic)
+static int reshard_engine(const DeriveFrom& f, uint32_t j, uint32_t G2, int kind, const dint_cfg& c, int device, dint_engine** out) {
+  const uint32_t G = (uint32_t)f.src.size();
+  return derive_engine(kind, c, device, j, f.rows[j], f.src, g_reshard_times, [&](dint_engine* e) {
+    const Ctx& d = e->ctx;
+    const cudaStream_t s = e->stream;
+    ReshardArgs a{};
+    a.G = G; a.G2 = G2; a.j = j; a.src_div = make_fastmod(G);
+    a.n_local = (uint32_t)e->total_groups;
+    a.n_global = kind == DINT_STORE ? e->kv[0].hash_size : e->cfg.lock_slots;
+    const int grid = e->sms * 4;
+    if (kind == DINT_LOCK2PL) {
+      for (uint32_t r = 0; r < G; r++) a.src[r] = (uint64_t)f.src[r]->ctx.cnt2;
+      a.dst = d.cnt2;
+      k_reshard_lock<K_LOCK2PL><<<grid, kThreads, 0, s>>>(a);
+    } else if (kind == DINT_FASST) {
+      for (uint32_t r = 0; r < G; r++) { a.src[r] = (uint64_t)f.src[r]->ctx.ver; a.src_bits[r] = (uint64_t)f.src[r]->ctx.lockbits; }
+      a.dst = d.ver;
+      a.dst_bits = d.lockbits;
+      k_reshard_lock<K_FASST><<<grid, kThreads, 0, s>>>(a);
+    } else {
+      for (uint32_t r = 0; r < G; r++)
+        k_kv_move<40><<<e->sms * 8, 256, 0, s>>>(f.src[r]->ctx.tbl[0], d.tbl[0], KeepOwner{d.tbl[0].lock_mod, G2, j});
+      if (d.ecache) {                                  // the eBPF tier: its sets move whole; its counters start at zero
+        for (uint32_t r = 0; r < G; r++) a.src[r] = (uint64_t)f.src[r]->ctx.ecache;
+        a.dst = d.ecache;
+        k_reshard_sets<<<grid, kThreads, 0, s>>>(a);
+      }
+    }
+  }, out);
+}
 
+// ---- rebuilding lost tatp / smallbank shards (rebuild.cuh has the placement arithmetic) ----------------------------
 static std::string mask_names(uint32_t mask) {
   std::string s;
   for (uint32_t r = 0; r < 32; r++)
@@ -2459,88 +2491,42 @@ static int rebuild_check(int kind, const dint_cfg& cfg, uint32_t G, uint32_t los
   return DINT_OK;
 }
 
-struct RebuildFrom {
-  std::vector<dint_engine*> src;                     // per shard: the engine read (nullptr where lost)
+struct RebuildFrom : DeriveFrom {
   uint32_t G = 0, lost = 0;
-  uint64_t keys[kMaxShards][kMaxTables] = {};        // the rows each lost shard receives, per table
-  // may shard s hold keys of lost shard d: within two positions of it, either way round
-  bool near(uint32_t s, uint32_t d) const { const uint32_t a = (s + G - d) % G; return a <= 2 || a >= G - 2; }
+  RebuildFrom(const std::vector<dint_engine*>& eng, uint32_t G_, uint32_t lost_) : G(G_), lost(lost_) {
+    src = eng;
+    for (uint32_t r = 0; r < G; r++) if ((lost >> r) & 1u) src[r] = nullptr;
+  }
+  // the surviving shards that may hold keys of a lost shard of `dsts`: within two positions of it, either way round
+  std::vector<dint_engine*> near(uint32_t dsts) const {
+    std::vector<dint_engine*> out(G, nullptr);
+    for (uint32_t s = 0; s < G; s++)
+      for (uint32_t d = 0; d < G; d++) {
+        const uint32_t a = (s + G - d) % G;
+        if (((dsts >> d) & 1u) && (a <= 2 || a >= G - 2)) out[s] = src[s];
+      }
+    return out;
+  }
+  // rows: every surviving source's rows per (lost shard, table)
+  int count() {
+    return count_rows(*this, near(lost), [&](uint32_t s, const KvTable&) { return RebuildDests{make_fastmod(G), G, lost, s}; },
+                      "rebuild row count");
+  }
   RebuildKeep keep(uint32_t s, uint32_t d) const { return RebuildKeep{make_fastmod(G), G, lost, s, d}; }
 };
 
-// f.src / G / lost, then every surviving source's rows per (table, lost shard): one small copy per source shard
-static int rebuild_prepare(RebuildFrom& f, const std::vector<dint_engine*>& eng, uint32_t G, uint32_t lost) {
-  f.src = eng; f.G = G; f.lost = lost;
-  for (uint32_t r = 0; r < G; r++) if ((lost >> r) & 1u) f.src[r] = nullptr;
-  for (uint32_t s = 0; s < G; s++) {
-    const dint_engine* e = f.src[s];
-    bool reads = false;
-    for (uint32_t d = 0; d < G; d++) reads |= ((lost >> d) & 1u) && f.near(s, d);
-    if (!e || !reads) continue;
-    CU(cudaSetDevice(e->device));
-    unsigned long long* d = nullptr;
-    unsigned long long h[kMaxTables][kMaxShards] = {};
-    CU(cudaMalloc(&d, sizeof h));
-    cudaError_t ce = cudaMemset(d, 0, sizeof h);
-    for (uint32_t t = 0; t < e->ctx.n_tables && ce == cudaSuccess; t++) {
-      k_rebuild_count<<<e->sms * 4, kThreads>>>(e->ctx.tbl[t], f.keep(s, 0), d + t * kMaxShards);
-      ce = cudaGetLastError();
+// Lost shard j, filled from the surviving sources within two positions of it
+static int rebuild_engine(const RebuildFrom& f, uint32_t j, int kind, const dint_cfg& c, int device, dint_engine** out) {
+  const std::vector<dint_engine*> read = f.near(1u << j);
+  return derive_engine(kind, c, device, j, f.rows[j], read, g_rebuild_times, [&](dint_engine* e) {
+    for (uint32_t s = 0; s < f.G; s++) {
+      if (!read[s]) continue;
+      for (uint32_t t = 0; t < e->ctx.n_tables; t++) {
+        if (kind == DINT_SMALLBANK) k_kv_move<8><<<e->sms * 8, 256, 0, e->stream>>>(read[s]->ctx.tbl[t], e->ctx.tbl[t], f.keep(s, j));
+        else k_kv_move<40><<<e->sms * 8, 256, 0, e->stream>>>(read[s]->ctx.tbl[t], e->ctx.tbl[t], f.keep(s, j));
+      }
     }
-    if (ce == cudaSuccess) ce = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (ce != cudaSuccess) return set_err(DINT_EIO, "rebuild row count", ce);
-    for (uint32_t t = 0; t < kMaxTables; t++)
-      for (uint32_t j = 0; j < G; j++) f.keys[j][t] += h[t][j];
-  }
-  return DINT_OK;
-}
-
-// Lost shard j on `device`, with configuration c: created as dint_create would (every table at least large enough to
-// keep the rows it receives at <= 35 % load, so kv_maintain leaves it as it is), then filled from the surviving
-// sources within two positions of it by k_rebuild_rows on its own stream.  Lock words, holder keys, the log ring and the
-// statistics are those of a new engine.
-static int rebuild_engine(const RebuildFrom& f, uint32_t j, int kind, dint_cfg c, int device, dint_engine** out) {
-  *out = nullptr;
-  double t0 = img_now();
-  KvPlan P;
-  if (kv_plan(kind, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
-  for (uint32_t t = 0; t < P.nt; t++) {
-    const uint32_t lg = kv_fit_log2(P.lg[t], f.keys[j][t]);
-    if (lg > 34) return set_errf(DINT_EINVAL, "rebuild: shard %u table %u would receive %llu rows", j, t, (unsigned long long)f.keys[j][t]);
-    c.kv_capacity_log2[t] = lg;
-  }
-  dint_engine* e = nullptr;
-  { int rc = dint_create(kind, &c, device, &e); if (rc) return rc; }
-  struct Owner { dint_engine* e; ~Owner() { if (e) dint_destroy(e); } } own{e};
-  for (uint32_t s = 0; s < f.G; s++)
-    if (f.src[s] && f.near(s, j)) { int rc = peer_enable(device, f.src[s]->device); if (rc) return rc; }
-  g_rebuild_times[2] += img_now() - t0;
-  const cudaStream_t st = e->stream;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  struct Events { cudaEvent_t* ev; ~Events() { for (int i = 0; i < 2; i++) if (ev[i]) cudaEventDestroy(ev[i]); } } evs{ev};
-  for (cudaEvent_t& x : ev) CU(cudaEventCreate(&x));
-  CU(cudaEventRecord(ev[0], st));
-  for (uint32_t s = 0; s < f.G; s++) {
-    if (!f.src[s] || !f.near(s, j)) continue;
-    const Ctx& from = f.src[s]->ctx;
-    for (uint32_t t = 0; t < e->ctx.n_tables; t++) {
-      if (kind == DINT_SMALLBANK) k_rebuild_rows<8><<<e->sms * 8, 256, 0, st>>>(from.tbl[t], e->ctx.tbl[t], f.keep(s, j));
-      else k_rebuild_rows<40><<<e->sms * 8, 256, 0, st>>>(from.tbl[t], e->ctx.tbl[t], f.keep(s, j));
-    }
-  }
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(ev[1], st));
-  CU(cudaEventSynchronize(ev[1]));
-  float ms = 0;
-  CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-  g_rebuild_times[1] += ms * 1e-3;
-  { int rc = kv_maintain(e, st); if (rc) return rc; }     // the host mirror of {live, used}, as reshard_engine
-  { int rc = kv_publish_counts(e, st); if (rc) return rc; }
-  CU(cudaStreamSynchronize(st));
-  e->stats = dint_stats{};
-  own.e = nullptr;
-  *out = e;
-  return DINT_OK;
+  }, out);
 }
 
 // dint_cluster_create; with image_dir dint_cluster_image_open: then shard r's engine is opened from its image; with
@@ -2548,7 +2534,7 @@ static int rebuild_engine(const RebuildFrom& f, uint32_t j, int kind, dint_cfg c
 // `rebuild` (dint_cluster_image_open_rebuild): the shards of *rebuild (known missing) and those whose image fails with
 // DINT_EIO are rebuilt from the others once those are open; *rebuild is then set to every shard rebuilt.
 static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* devices, uint64_t max_batch, const char* image_dir,
-                        const ReshardFrom* from, uint32_t* rebuild, dint_cluster** out) {
+                        const DeriveFrom* from, uint32_t* rebuild, dint_cluster** out) {
   if (!out || kind < 0 || kind >= DINT_NUM_KINDS || n_gpus < 1 || n_gpus > kMaxShards) return set_err(DINT_EINVAL, "bad kind / n_gpus");
   *out = nullptr;
   const bool by_dst = kind == DINT_TATP || kind == DINT_SMALLBANK;
@@ -2590,7 +2576,7 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     dint_engine* e = nullptr;
     if (rebuild && ((*rebuild >> r) & 1u)) { failed |= 1u << r; cl->eng.push_back(nullptr); continue; }   // known missing
     rc = image_dir ? image_open_impl(img_shard_path(image_dir, r).c_str(), cl->dev[r], &c, &e)
-         : from    ? reshard_engine(*from, r, G, c, cl->dev[r], &e)
+         : from    ? reshard_engine(*from, r, G, kind, c, cl->dev[r], &e)
                    : dint_create(kind, &c, cl->dev[r], &e);
     if (rc == DINT_EIO && rebuild) {                    // a short, unreadable or corrupt image: rebuilt below
       failed |= 1u << r;
@@ -2602,8 +2588,8 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     rc = rebuild_check(kind, base, G, failed);
     if (rc) rc = set_errf(DINT_EIO, "image %s: shard image(s) %s failed and cannot be rebuilt: %s", image_dir,
                           mask_names(failed).c_str(), g_last_error.c_str());
-    RebuildFrom f;
-    if (rc == DINT_OK) rc = rebuild_prepare(f, cl->eng, G, failed);
+    RebuildFrom f(cl->eng, G, failed);
+    if (rc == DINT_OK) rc = f.count();
     for (uint32_t r = 0; r < G && rc == DINT_OK; r++)
       if ((failed >> r) & 1u) rc = rebuild_engine(f, r, kind, cluster_shard_cfg(cl, r), cl->dev[r], &cl->eng[r]);
     if (rc == DINT_OK) *rebuild = failed;
@@ -2615,21 +2601,9 @@ static int cluster_make(int kind, const dint_cfg* cfg, int n_gpus, const int* de
     if (cudaSetDevice(cl->dev[r]) != cudaSuccess || cudaMalloc(&p, 2 * S * region + 4096) != cudaSuccess) { rc = set_err(DINT_ENOMEM, "cluster buffers", cudaGetLastError()); break; }
     cudaMemset(p, 0, 2 * S * region + 4096);
     cl->bufs.push_back(p);
-    if (!cl->shared_device)
-      for (uint32_t q = 0; q < G; q++)
-        if (q != r) {
-          int can = 0;
-          cudaDeviceCanAccessPeer(&can, cl->dev[r], cl->dev[q]);
-          if (!can) { rc = set_err(DINT_ENODEV, "GPUs without peer access"); break; }
-          cudaError_t ce = cudaDeviceEnablePeerAccess(cl->dev[q], 0);
-          if (ce != cudaSuccess && ce != cudaErrorPeerAccessAlreadyEnabled) { rc = set_err(DINT_EIO, "cudaDeviceEnablePeerAccess", ce); break; }
-          cudaGetLastError();
-        }
+    for (uint32_t q = 0; q < G && rc == DINT_OK; q++) rc = peer_enable(cl->dev[r], cl->dev[q]);
   }
-  for (uint32_t r = 0; r < G && rc == DINT_OK; r++) {
-    cudaSetDevice(cl->dev[r]);
-    cudaDeviceSynchronize();
-  }
+  if (rc == DINT_OK) cluster_quiesce(cl);
   if (rc == DINT_OK) rc = cluster_ranks(cl, cl->eng, cl->sh);
   if (rc != DINT_OK) { std::string keep = g_last_error; dint_cluster_destroy(cl); g_last_error = keep; return rc; }
   *out = cl;
@@ -2731,13 +2705,10 @@ int dint_cluster_rebuild(dint_cluster* cl, uint32_t lost_mask) {
                                  "shards do not, so destroy them first", cl->txn_clients);
   for (double& t : g_rebuild_times) t = 0;
   const double t0 = img_now();
-  for (uint32_t r = 0; r < cl->G; r++) {               // quiesce every device, as dint_cluster_reshard does
-    CU(cudaSetDevice(cl->dev[r]));
-    CU(cudaDeviceSynchronize());
-  }
+  { int rc = cluster_quiesce(cl); if (rc) return rc; }
   const uint32_t G = cl->G;
-  RebuildFrom f;
-  { int rc = rebuild_prepare(f, cl->eng, G, lost_mask); if (rc) return rc; }
+  RebuildFrom f(cl->eng, G, lost_mask);
+  { int rc = f.count(); if (rc) return rc; }
   g_rebuild_times[2] += img_now() - t0;
   // the new engines and rank contexts are made next to the old ones, so a failure leaves the cluster as it was
   std::vector<dint_engine*> eng = cl->eng;
@@ -2771,10 +2742,7 @@ int dint_cluster_rebuild(dint_cluster* cl, uint32_t lost_mask) {
   }
   cl->eng = eng;
   cl->sh = sh;
-  for (uint32_t r = 0; r < G; r++) {
-    CU(cudaSetDevice(cl->dev[r]));
-    CU(cudaDeviceSynchronize());
-  }
+  { int rc = cluster_quiesce(cl); if (rc) return rc; }
   g_rebuild_times[0] = img_now() - t0;
   return DINT_OK;
 }
@@ -2796,13 +2764,11 @@ int dint_cluster_reshard(dint_cluster* src, int n_gpus, const int* devices, uint
   if (n_gpus < 1 || n_gpus > kMaxShards) return set_err(DINT_EINVAL, "bad n_gpus");
   for (double& t : g_reshard_times) t = 0;
   const double t0 = img_now();
-  for (uint32_t r = 0; r < src->G; r++) {              // quiesce the source, as dint_snapshot_create does
-    CU(cudaSetDevice(src->dev[r]));
-    CU(cudaDeviceSynchronize());
-  }
-  ReshardFrom f;
-  f.src = src;
-  { int rc = reshard_count_keys(f, (uint32_t)n_gpus); if (rc) return rc; }
+  { int rc = cluster_quiesce(src); if (rc) return rc; }   // as dint_snapshot_create quiesces an engine
+  DeriveFrom f;
+  f.src = src->eng;
+  const uint32_t G2 = (uint32_t)n_gpus;
+  { int rc = count_rows(f, f.src, [&](uint32_t, const KvTable& t) { return OwnerDests{t.lock_mod, G2, (1u << G2) - 1}; }, "re-shard key count"); if (rc) return rc; }
   g_reshard_times[2] += img_now() - t0;
   const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, nullptr, out);
   g_reshard_times[0] = img_now() - t0;

@@ -13,17 +13,17 @@
 // EMPTY inside a launch, so a probe sequence that reaches EMPTY proves absence.  Deletes leave tombstones
 // (an insert reuses the first one on its probe path); the engine counts the entries that have left EMPTY
 // (`live[1]`) and, between calls, rehashes a table into a fresh array once FULL + TOMB passes 70 % of its
-// capacity (k_kv_rehash, engine.cu kv_maintain) -- the reference's chained kvs frees entries on delete
+// capacity (k_kv_move, engine.cu kv_maintain) -- the reference's chained kvs frees entries on delete
 // (store/udp/kvs.h:124-133), so without this a long insert/delete churn would grow the probe chains without
 // bound.  Requests on the same key are never
 // concurrent (same group -> K3 replays them in one thread); requests on different keys only meet on
 // the `meta` word, which is claimed with atomicCAS.
 #pragma once
 #include <functional>
-#include <type_traits>
 #include "engine.cuh"
 #ifdef __CUDACC__
 #include <cooperative_groups.h>
+#include "kernels.cuh"
 #endif
 
 namespace dint {
@@ -1133,12 +1133,12 @@ __global__ void __launch_bounds__(256) k_kv_load(const Ctx c, int table, const u
   if (!kv_insert_words<VALSZ>(t, key, h, w)) atomicAdd(&c.counters[0], 1ULL);
 }
 
-// Every FULL entry of `from` is inserted into `to` with its version; tombstones vanish.  `from` may sit in a peer
-// device's memory, and the caller sizes `to` for every key it receives.  Filters: with n_owners > 1 (a re-shard,
-// reshard.cuh) only the entries whose global group (fasthash64(key) % to.lock_mod, the reference's bucket) is owned by
-// shard `owner` of n_owners; with a Keep (a rebuild, rebuild.cuh) only the entries for which keep(key) holds.
-template <int VALSZ, class Keep = void>
-DINT_D void kv_move_rows(const KvTable& from, const KvTable& to, uint32_t n_owners, uint32_t owner, const Keep* keep = nullptr) {
+// Every FULL entry of `from` for which keep(key, fasthash64(key)) holds is inserted into `to` with its version;
+// tombstones vanish.  `from` may sit in a peer device's memory, and the caller sizes `to` for every key it receives.
+// Filters: KeepAll (the tombstone rehash, kv_maintain), KeepOwner (a re-shard, reshard.cuh), RebuildKeep (a rebuild,
+// rebuild.cuh).
+template <int VALSZ, class Keep>
+__global__ void __launch_bounds__(256) k_kv_move(const KvTable from, const KvTable to, const Keep keep) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= from.cap_mask; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t* e = from.entries + (i << from.ent_shift);
     uint4 v[Ent<VALSZ>::NV];
@@ -1146,11 +1146,7 @@ DINT_D void kv_move_rows(const KvTable& from, const KvTable& to, uint32_t n_owne
     if (v[0].w != ENT_FULL) continue;
     const uint64_t key = ((uint64_t)v[0].y << 32) | v[0].x;
     const uint64_t h = fasthash64_u64(key);
-    if constexpr (std::is_void_v<Keep>) {
-      if (n_owners > 1 && fast_mod(h, to.lock_mod) % n_owners != owner) continue;
-    } else {
-      if (!(*keep)(key)) continue;
-    }
+    if (!keep(key, h)) continue;
     uint32_t w[Ent<VALSZ>::NW];
     const uint32_t* flat = (const uint32_t*)v;
 #pragma unroll
@@ -1158,11 +1154,34 @@ DINT_D void kv_move_rows(const KvTable& from, const KvTable& to, uint32_t n_owne
     kv_insert_words<VALSZ>(to, key, h, w, v[0].z);   // (`to` has room for every key it receives: cannot fail)
   }
 }
+struct KeepAll {
+  DINT_D bool operator()(uint64_t, uint64_t) const { return true; }
+};
 
-// Rehash of one table into a fresh (zeroed) array, or (n_owners > 1) one source table's share of a re-shard.
-template <int VALSZ>
-__global__ void __launch_bounds__(256) k_kv_rehash(const KvTable from, const KvTable to, uint32_t n_owners, uint32_t owner) {
-  kv_move_rows<VALSZ>(from, to, n_owners, owner);
+// out[d] += the FULL entries of table t that go to destination shard d, for every d of dests.all: dests(key,
+// fasthash64(key)) is the bit mask of a row's destinations (OwnerDests, reshard.cuh; RebuildDests, rebuild.cuh).
+// Destination tables are sized from these counts before a single row is inserted.
+template <class Dests>
+__global__ void __launch_bounds__(kThreads) k_kv_count_rows(const KvTable t, const Dests dests, unsigned long long* out) {
+  __shared__ unsigned long long s_cnt[kMaxShards];
+  if (threadIdx.x < kMaxShards) s_cnt[threadIdx.x] = 0;
+  __syncthreads();
+  const uint64_t end = (t.cap_mask + 32) / 32 * 32;              // whole warps: the ballots below need every lane
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t m = 0;
+    if (i <= t.cap_mask) {
+      const uint4 v = __ldcg((const uint4*)(t.entries + (i << t.ent_shift)));   // {key, ver, meta}
+      const uint64_t key = ((uint64_t)v.y << 32) | v.x;
+      if (v.w == ENT_FULL) m = dests(key, fasthash64_u64(key));
+    }
+    for (uint32_t a = dests.all; a; a &= a - 1) {
+      const uint32_t d = __ffs(a) - 1;
+      const uint32_t n = __popc(__ballot_sync(0xffffffffu, (m >> d) & 1u));
+      if (n && lane_id() == 0) atomicAdd(&s_cnt[d], (unsigned long long)n);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < kMaxShards && s_cnt[threadIdx.x]) atomicAdd(&out[threadIdx.x], s_cnt[threadIdx.x]);
 }
 
 // valid slots of table `table`'s chain entries (dint_kv_count with the eBPF tier): freed entries hold none

@@ -6,19 +6,19 @@
 // numbering the other way, so destination shard j, local g', is global s = g' G' + j, read from source shard s % G at
 // local s / G.  Every destination element is found from its own global id: the gathers below write each destination
 // word exactly once, need no atomics and give the same bytes whatever the launch order.  The only atomics are those of
-// the KV inserts (kv_insert_words, through k_kv_rehash), which claim free table entries.
+// the KV inserts (kv_insert_words, through k_kv_move), which claim free table entries.
 //
 //   k_reshard_lock    lock_2pl {num_ex, num_sh} per group, or lock_fasst's version per group and its lock bits: one
 //                     bit per local group, gathered 32 destination groups per warp and stored as one word (ballot).
 //                     A lock held before the move is held after it.
 //   k_reshard_sets    the store's eBPF cache tier: one 256-byte set per bucket moves whole (keys, versions, valid and
 //                     dirty masks, bloom word, values), 16 threads per set.
-//   k_kv_owner_count  the store's FULL table entries per destination shard (bucket % G'), so that every destination
-//                     table is sized to hold its keys before a single one is inserted.
-//   the store's table entries move through k_kv_rehash (kv.cuh) with an owner filter: one pass per (source table,
-//   destination), each FULL entry inserted with its version; tombstones are dropped and {live, used} recounted.
+//   the store's table entries are first counted per destination shard (bucket % G') by k_kv_count_rows (kv.cuh) with
+//   OwnerDests, so that every destination table is sized to hold its keys before a single one is inserted, then move
+//   through k_kv_move (kv.cuh) with KeepOwner: one pass per (source table, destination), each FULL entry inserted with
+//   its version; tombstones are dropped and {live, used} recounted.
 //
-// The kernels run on the destination's device; a source shard on another GPU is read through peer memory.
+// The gathers and k_kv_move run on the destination's device; a source shard on another GPU is read through peer memory.
 #pragma once
 #include "kernels.cuh"
 #include "kv.cuh"
@@ -34,6 +34,22 @@ struct ReshardArgs {
   uint64_t n_global;               // global lock slots (lock kinds) or buckets (store)
   void* dst;
   uint32_t* dst_bits;              // lock_fasst
+};
+
+// A store key's bucket is fasthash64(key) % the table's bucket count (bucket_mod); destination shard bucket % n owns it.
+struct KeepOwner {                 // k_kv_move: the keys destination shard `owner` of n receives
+  FastMod bucket_mod;
+  uint32_t n, owner;
+#ifdef __CUDACC__
+  DINT_D bool operator()(uint64_t, uint64_t h) const { return fast_mod(h, bucket_mod) % n == owner; }
+#endif
+};
+struct OwnerDests {                // k_kv_count_rows: every key to its owner of n; all = (1 << n) - 1
+  FastMod bucket_mod;
+  uint32_t n, all;
+#ifdef __CUDACC__
+  DINT_D uint32_t operator()(uint64_t, uint64_t h) const { return 1u << (fast_mod(h, bucket_mod) % n); }
+#endif
 };
 
 #ifdef __CUDACC__
@@ -76,25 +92,6 @@ __global__ void __launch_bounds__(kThreads) k_reshard_sets(const ReshardArgs a) 
     if (!reshard_src(a, t / kVecs, r, l)) continue;
     ((uint4*)a.dst)[t] = __ldcg((const uint4*)a.src[r] + l * kVecs + t % kVecs);
   }
-}
-
-// out[o] += the FULL entries of table t whose bucket (fasthash64(key) % t.lock_mod) is owned by shard o of n_owners
-__global__ void __launch_bounds__(kThreads) k_kv_owner_count(const KvTable t, uint32_t n_owners, unsigned long long* out) {
-  __shared__ unsigned long long s_cnt[kMaxShards];
-  if (threadIdx.x < kMaxShards) s_cnt[threadIdx.x] = 0;
-  __syncthreads();
-  const uint64_t end = (t.cap_mask + 32) / 32 * 32;              // whole warps: the match below needs every lane
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (uint64_t)gridDim.x * blockDim.x) {
-    uint32_t o = 0xffu;
-    if (i <= t.cap_mask) {
-      const uint4 v = __ldcg((const uint4*)(t.entries + (i << t.ent_shift)));   // {key, ver, meta}
-      if (v.w == ENT_FULL) o = fast_mod(fasthash64_u64(((uint64_t)v.y << 32) | v.x), t.lock_mod) % n_owners;
-    }
-    const uint32_t peers = __match_any_sync(0xffffffffu, o);
-    if (o < kMaxShards && (int)lane_id() == __ffs(peers) - 1) atomicAdd(&s_cnt[o], (unsigned long long)__popc(peers));
-  }
-  __syncthreads();
-  if (threadIdx.x < n_owners && s_cnt[threadIdx.x]) atomicAdd(&out[threadIdx.x], s_cnt[threadIdx.x]);
 }
 #endif  // __CUDACC__
 
