@@ -600,6 +600,10 @@ uint32_t dint_test_fastmod(uint64_t n, uint32_t d) { FastMod f = make_fastmod(d)
 int dint_test_rebuild_source(uint64_t key, uint32_t G, uint32_t lost_mask) {
   return G == 0 || G > kMaxShards ? -1 : rebuild_source((uint32_t)(key % G), G, lost_mask);
 }
+uint32_t dint_test_txn_reshard_dests(uint64_t key, uint32_t G, uint32_t G2, uint32_t src) {
+  if (G == 0 || G > kMaxShards || G2 == 0 || G2 > kMaxShards) return 0;
+  return ReplicaDests{make_fastmod(G), make_fastmod(G2), G2, (1u << G2) - 1, src}(key, 0);
+}
 uint32_t dint_test_host_slices(uint64_t n, uint32_t min_slice, uint32_t max_slice, int ramp_up, uint32_t* out, uint32_t cap) {
   HostSlices sched(n, min_slice, max_slice, ramp_up != 0);
   uint32_t k = 0;
@@ -2404,9 +2408,10 @@ static int derive_engine(int kind, dint_cfg c, int device, uint32_t j, const uin
     if (kv_plan(kind, c, false, P) != DINT_OK) return set_err(DINT_EINVAL, "bad KV configuration");
     for (uint32_t t = 0; t < P.nt; t++) {
       const uint32_t lg = kv_fit_log2(P.lg[t], rows[t]);
-      if (lg > 34)                                     // (a store is re-sharded; tatp and smallbank are rebuilt)
+      if (lg > 34)
         return kind == DINT_STORE ? set_errf(DINT_EINVAL, "re-shard: shard %u would receive %llu keys", j, (unsigned long long)rows[t])
-                                  : set_errf(DINT_EINVAL, "rebuild: shard %u table %u would receive %llu rows", j, t, (unsigned long long)rows[t]);
+                                  : set_errf(DINT_EINVAL, "%s: shard %u table %u would receive %llu rows",
+                                             times == g_rebuild_times ? "rebuild" : "re-shard", j, t, (unsigned long long)rows[t]);
       c.kv_capacity_log2[t] = lg;
     }
   }
@@ -2434,7 +2439,7 @@ static int derive_engine(int kind, dint_cfg c, int device, uint32_t j, const uin
 }
 
 // Destination shard j of G2, filled from every source shard by the kernels of reshard.cuh (which has the ownership
-// arithmetic)
+// arithmetic); tatp / smallbank with ReplicaKeep (rebuild.cuh, which has the replica arithmetic)
 static int reshard_engine(const DeriveFrom& f, uint32_t j, uint32_t G2, int kind, const dint_cfg& c, int device, dint_engine** out) {
   const uint32_t G = (uint32_t)f.src.size();
   return derive_engine(kind, c, device, j, f.rows[j], f.src, g_reshard_times, [&](dint_engine* e) {
@@ -2454,6 +2459,13 @@ static int reshard_engine(const DeriveFrom& f, uint32_t j, uint32_t G2, int kind
       a.dst = d.ver;
       a.dst_bits = d.lockbits;
       k_reshard_lock<K_FASST><<<grid, kThreads, 0, s>>>(a);
+    } else if (kind == DINT_TATP || kind == DINT_SMALLBANK) {
+      for (uint32_t r = 0; r < G; r++)
+        for (uint32_t t = 0; t < d.n_tables; t++) {
+          const ReplicaKeep keep{make_fastmod(G), make_fastmod(G2), G2, r, j};
+          if (kind == DINT_SMALLBANK) k_kv_move<8><<<e->sms * 8, 256, 0, s>>>(f.src[r]->ctx.tbl[t], d.tbl[t], keep);
+          else k_kv_move<40><<<e->sms * 8, 256, 0, s>>>(f.src[r]->ctx.tbl[t], d.tbl[t], keep);
+        }
     } else {
       for (uint32_t r = 0; r < G; r++)
         k_kv_move<40><<<e->sms * 8, 256, 0, s>>>(f.src[r]->ctx.tbl[0], d.tbl[0], KeepOwner{d.tbl[0].lock_mod, G2, j});
@@ -2476,12 +2488,13 @@ static std::string mask_names(uint32_t mask) {
 
 // DINT_EINVAL, with the reason, unless the shards of `lost` of a G-shard cluster of this kind and configuration can be
 // rebuilt from the others
+static const char kEbpfRows[] = "the eBPF cache tiers hold dirty and cache-only rows whose wire-visible versions depend on "
+                                "each shard's own hit history";
 static int rebuild_check(int kind, const dint_cfg& cfg, uint32_t G, uint32_t lost) {
   if (kind != DINT_TATP && kind != DINT_SMALLBANK)
     return set_err(DINT_EINVAL, "rebuild: lock_2pl, lock_fasst, store and log_server clusters keep no replicas");
   if (cfg.flags & (DINT_CFG_TATP_EBPF | DINT_CFG_SMALLBANK_EBPF))
-    return set_err(DINT_EINVAL, "rebuild: the eBPF cache tiers hold dirty and cache-only rows whose wire-visible versions depend on "
-                                "each shard's own hit history, so no peer's copy is that shard's state");
+    return set_errf(DINT_EINVAL, "rebuild: %s, so no peer's copy is that shard's state", kEbpfRows);
   if (G < 3) return set_err(DINT_EINVAL, "rebuild: a one-shard cluster has no replica to rebuild from");
   if (lost == 0 || (lost >> G) != 0) return set_errf(DINT_EINVAL, "rebuild: lost mask 0x%x is empty or names shards outside [0, %u)", lost, G);
   for (uint32_t p = 0; p < G; p++)
@@ -2769,6 +2782,50 @@ int dint_cluster_reshard(dint_cluster* src, int n_gpus, const int* devices, uint
   f.src = src->eng;
   const uint32_t G2 = (uint32_t)n_gpus;
   { int rc = count_rows(f, f.src, [&](uint32_t, const KvTable& t) { return OwnerDests{t.lock_mod, G2, (1u << G2) - 1}; }, "re-shard key count"); if (rc) return rc; }
+  g_reshard_times[2] += img_now() - t0;
+  const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, nullptr, out);
+  g_reshard_times[0] = img_now() - t0;
+  return rc;
+}
+
+int dint_cluster_reshard_txn(dint_cluster* src, int n_gpus, const int* devices, uint64_t max_batch, dint_cluster** out) {
+  if (!src || !out) return set_err(DINT_EINVAL, "null argument");
+  *out = nullptr;
+  if (src->kind != DINT_TATP && src->kind != DINT_SMALLBANK)
+    return set_err(DINT_EINVAL, "re-shard: dint_cluster_reshard_txn re-places tatp and smallbank replicas; lock_2pl, lock_fasst "
+                                "and store clusters re-shard with dint_cluster_reshard, and a log_server record has no key");
+  if (src->base.flags & (DINT_CFG_TATP_EBPF | DINT_CFG_SMALLBANK_EBPF))
+    return set_errf(DINT_EINVAL, "re-shard: %s, so no one shard's table holds a key's row", kEbpfRows);
+  if (n_gpus < 1 || n_gpus == 2 || n_gpus > (int)kMaxShards)
+    return set_errf(DINT_EINVAL, "re-shard: %d shards; tatp / smallbank placement needs 1 or 3..8 (primary + 2 backups)", n_gpus);
+  for (double& t : g_reshard_times) t = 0;
+  const double t0 = img_now();
+  { int rc = cluster_quiesce(src); if (rc) return rc; }
+  const uint32_t G = src->G, G2 = (uint32_t)n_gpus;
+  // a held lock means a client is mid-transaction: its rows may differ between replicas, and the lock would be lost
+  for (uint32_t r = 0; r < G; r++) {
+    const dint_engine* e = src->eng[r];
+    CU(cudaSetDevice(e->device));
+    unsigned long long* d = nullptr;
+    unsigned long long held = 0;
+    CU(cudaMalloc(&d, sizeof held));
+    cudaError_t ce = cudaMemset(d, 0, sizeof held);
+    if (ce == cudaSuccess) {
+      k_locks_held<<<e->sms * 4, kThreads>>>(src->kind == DINT_TATP ? e->ctx.lockbits : nullptr,
+                                             src->kind == DINT_SMALLBANK ? e->ctx.cnt2 : nullptr, e->total_groups, d);
+      ce = cudaGetLastError();
+    }
+    if (ce == cudaSuccess) ce = cudaMemcpy(&held, d, sizeof held, cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    if (ce != cudaSuccess) return set_err(DINT_EIO, "re-shard lock count", ce);
+    if (held)
+      return set_errf(DINT_EINVAL, "re-shard: shard %u holds %llu locks: clients are mid-transaction, drain them first "
+                                   "(dint_txn_clients_drain)", r, held);
+  }
+  DeriveFrom f;
+  f.src = src->eng;
+  { int rc = count_rows(f, f.src, [&](uint32_t s, const KvTable&) { return ReplicaDests{make_fastmod(G), make_fastmod(G2), G2, (1u << G2) - 1, s}; },
+                        "re-shard row count"); if (rc) return rc; }
   g_reshard_times[2] += img_now() - t0;
   const int rc = cluster_make(src->kind, &src->base, n_gpus, devices, max_batch, nullptr, &f, nullptr, out);
   g_reshard_times[0] = img_now() - t0;
@@ -3130,13 +3187,15 @@ static int serve_rounds(RoundLoop& L, std::vector<Rank>& rk, uint32_t rounds, Em
   auto t_prev = std::chrono::steady_clock::now();
   for (uint32_t i = 0; i < rounds; i++) {
     // the slab capacity of the round: the largest (source, owner) count, so no slab can overflow
-    uint64_t maxc = 0;
+    uint64_t maxc = 0, total = 0;
     bool fits = true;
     for (uint32_t r = 0; r < G; r++) {
       n[r] = rk[r].pub[0];
+      total += n[r];
       if (n[r] > cl->max_n) fits = false;
       for (uint32_t o = 0; o < G; o++) maxc = rk[r].pub[1 + o] > maxc ? rk[r].pub[1 + o] : maxc;
     }
+    if (total == 0) break;                      // the end of a drain (dint_txn_clients_drain): not served, not counted
     if (maxc > cl->cap) fits = false;
     b.assign(G, {});
     if (L.local) {
@@ -3207,6 +3266,7 @@ struct TxnRank : RoundRank {
 };
 struct dint_txn_clients : RoundLoop {
   uint32_t n = 0;
+  bool drained = false;          // the pending round is empty after a drain: the next run / peek / stats resumes
   std::vector<TxnRank> rk;
 };
 
@@ -3309,14 +3369,93 @@ static int txn_emit(dint_txn_clients* t, int first) {
   return DINT_OK;
 }
 
+// the first emission (every client starts), or after a drain the one that resumes the clients: every idle client
+// begins its next transaction and emits its first records
+static int txn_start(dint_txn_clients* t) {
+  if (!t->started) return txn_emit(t, 1);
+  if (!t->drained) return DINT_OK;
+  t->drained = false;
+  return txn_emit(t, 0);
+}
+
 int dint_txn_clients_run(dint_txn_clients* t, uint32_t rounds) {
   if (!t) return set_err(DINT_EINVAL, "null argument");
+  { int rc = txn_start(t); if (rc) return rc; }
   return serve_rounds(*t, t->rk, rounds, [t](int first) { return txn_emit(t, first); });
+}
+
+int dint_txn_clients_drain(dint_txn_clients* t, uint32_t max_rounds, uint32_t* rounds) {
+  if (!t) return set_err(DINT_EINVAL, "null argument");
+  if (rounds) *rounds = 0;
+  if (!t->started || t->drained) return DINT_OK;       // nothing pending
+  for (TxnRank& k : t->rk) k.d.w.drain = 1;
+  const uint64_t before = t->rounds;
+  int rc = serve_rounds(*t, t->rk, max_rounds, [t](int first) { return txn_emit(t, first); });
+  for (TxnRank& k : t->rk) k.d.w.drain = 0;            // (an idle client resumes at the next emission)
+  if (rounds) *rounds = (uint32_t)(t->rounds - before);
+  if (rc && rc != DINT_EPROTO) return rc;
+  uint64_t pending = 0;                                // serve_rounds waited for the last emission
+  for (const TxnRank& k : t->rk) pending += k.pub[0];
+  if (pending == 0) {
+    t->drained = true;
+    return rc;
+  }
+  uint64_t busy = 0;                                   // a client is busy while it emits records
+  for (uint32_t r = 0; r < t->cl->G; r++) {
+    std::vector<uint32_t> cnt(t->rk[r].d.n);
+    CU(cudaSetDevice(t->cl->dev[r]));
+    if (!cnt.empty()) CU(cudaMemcpy(cnt.data(), t->rk[r].d.cnt, cnt.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t c : cnt) busy += c != 0;
+  }
+  return set_errf(DINT_EINVAL, "drain: %llu clients are still mid-transaction after %u rounds", (unsigned long long)busy, max_rounds);
+}
+
+int dint_txn_clients_rebind(dint_txn_clients* t, dint_cluster* c) {
+  if (!t || !c) return set_err(DINT_EINVAL, "null argument");
+  if (c->kind != t->cl->kind) return set_err(DINT_EINVAL, "rebind: the cluster serves another kind than these clients");
+  if (t->started && !t->drained)
+    return set_err(DINT_EINVAL, "rebind: the clients are mid-transaction (their pending round holds records): drain them first");
+  dint_txn_clients* n = nullptr;
+  { int rc = dint_txn_clients_create(c, t->n, (uint32_t)t->rk[0].d.gid0, t->rk[0].d.w.keys, &n); if (rc) return rc; }
+  auto fail = [&](int code) { std::string keep = g_last_error; dint_txn_clients_destroy(n); g_last_error = keep; return code; };
+  dint_cluster* old = t->cl;
+  for (uint32_t r = 0; r < old->G; r++)                // the last emission is done
+    if (cudaSetDevice(old->dev[r]) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)
+      return fail(set_err(DINT_EIO, "rebind: synchronise", cudaGetLastError()));
+  // each client's record moves block by block: every (old rank, new rank) pair's common range of client ids.  The
+  // pending round is empty, so no record of a round moves.
+  const size_t csz = c->kind == DINT_TATP ? sizeof(txn::TatpClient) : sizeof(txn::SbClient);
+  unsigned long long sum[txn::kDevStats] = {0};
+  for (uint32_t r = 0; r < old->G; r++) {
+    const txn::DevClients& f = t->rk[r].d;
+    unsigned long long h[txn::kDevStats];
+    if (cudaSetDevice(old->dev[r]) != cudaSuccess || cudaMemcpy(h, f.stats, sizeof h, cudaMemcpyDeviceToHost) != cudaSuccess)
+      return fail(set_err(DINT_EIO, "rebind: counters", cudaGetLastError()));
+    for (uint32_t i = 0; i < txn::kDevStats; i++) sum[i] += h[i];
+    for (uint32_t q = 0; q < c->G; q++) {
+      const txn::DevClients& to = n->rk[q].d;
+      const uint64_t lo = std::max(f.gid0, to.gid0), hi = std::min(f.gid0 + f.n, to.gid0 + to.n);
+      if (lo < hi && cudaMemcpyPeer((uint8_t*)to.cl + (lo - to.gid0) * csz, c->dev[q], (const uint8_t*)f.cl + (lo - f.gid0) * csz,
+                                    old->dev[r], (hi - lo) * csz) != cudaSuccess)
+        return fail(set_err(DINT_EIO, "rebind: client state", cudaGetLastError()));
+    }
+  }
+  // the counters carry over: the stats sum the ranks, so the new rank 0 holds the old sums
+  if (cudaSetDevice(c->dev[0]) != cudaSuccess || cudaMemcpy(n->rk[0].d.stats, sum, sizeof sum, cudaMemcpyHostToDevice) != cudaSuccess)
+    return fail(set_err(DINT_EIO, "rebind: counters", cudaGetLastError()));
+  // t takes the new ranks; n takes the old ones and releases them, and its attachment, on the old cluster
+  std::swap(t->cl, n->cl);
+  std::swap(t->rk, n->rk);
+  std::swap(t->mains, n->mains);
+  std::swap(t->t_beg, n->t_beg);
+  std::swap(t->t_end, n->t_end);
+  dint_txn_clients_destroy(n);
+  return DINT_OK;
 }
 
 // the ranks' DevClients::stats words, summed (synchronises)
 static int txn_dev_stats(dint_txn_clients* t, unsigned long long by[txn::kDevStats]) {
-  if (!t->started) { int rc = txn_emit(t, 1); if (rc) return rc; }
+  { int rc = txn_start(t); if (rc) return rc; }
   for (uint32_t i = 0; i < txn::kDevStats; i++) by[i] = 0;
   for (uint32_t r = 0; r < t->cl->G; r++) {
     unsigned long long h[txn::kDevStats];
@@ -3360,7 +3499,7 @@ int dint_txn_clients_lock_stats(dint_txn_clients* t, uint64_t out[3]) {
 int dint_txn_clients_peek(dint_txn_clients* t, void* next_req, uint8_t* next_dst, uint64_t* n_next, void* last_resp, uint64_t* n_last) {
   if (!t) return set_err(DINT_EINVAL, "null argument");
   int rc;
-  if (!t->started && (rc = txn_emit(t, 1))) return rc;
+  if ((rc = txn_start(t))) return rc;
   if ((rc = round_wait(*t, t->rk))) return rc;
   uint64_t a = 0, z = 0;
   for (uint32_t r = 0; r < t->cl->G; r++) {

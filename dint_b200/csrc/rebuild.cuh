@@ -14,6 +14,16 @@
 //
 // k_kv_move runs on the destination's device; a source shard on another GPU is read through peer memory.  Only the
 // sources within two positions of a lost shard hold its keys, and only those are read.
+//
+// Re-placing onto another shard count (dint_cluster_reshard_txn).  At a drained point every replica of a key holds the
+// same row; the source of key k is its old primary, shard k % G, so the result does not depend on the launch order.
+// Destination shard j of G' receives every key it replicates under G', (k % G' + i) % G' for i = 0, 1, 2 (for G' = 1
+// only shard 0; each key still gets one row).
+//
+//   ReplicaDests   k_kv_count_rows's filter: the destinations of one source's primary rows.
+//   ReplicaKeep    k_kv_move's filter: one source's primary rows that destination dst replicates.
+//   k_locks_held   the held lock groups of one shard: the call refuses a source with any, since a client that holds a
+//                  lock is mid-transaction and its replicas may differ.
 #pragma once
 #include "kernels.cuh"
 #include "kv.cuh"
@@ -48,5 +58,49 @@ struct RebuildDests {
   }
 #endif
 };
+
+struct ReplicaKeep {
+  FastMod gmod, g2mod;             // G, G': the source and destination shard counts
+  uint32_t G2, src, dst;           // src: the shard read; dst: the destination shard filled
+#ifdef __CUDACC__
+  DINT_D bool operator()(uint64_t key, uint64_t) const {
+    return fast_mod(key, gmod) == src && txn_role(fast_mod(key, g2mod), G2, dst) <= 2;
+  }
+#endif
+};
+struct ReplicaDests {
+  FastMod gmod, g2mod;
+  uint32_t G2, all, src;           // all = (1 << G') - 1; src: the shard read
+  // the destinations of key's row when src is its old primary (also the host test hook's answer)
+  DINT_HD uint32_t operator()(uint64_t key, uint64_t) const {
+    if (fast_mod(key, gmod) != src) return 0;
+    const uint32_t p = fast_mod(key, g2mod);
+    uint32_t dests = 0;
+    for (uint32_t i = 0; i < 3; i++) dests |= 1u << ((p + i) % G2);
+    return dests;
+  }
+};
+
+#ifdef __CUDACC__
+// out += the held lock groups of one tatp / smallbank shard: the set bits of `bits` (tatp, one bit per group), or the
+// groups of `cnt2` (smallbank, {num_ex, num_sh}) that are not {0, 0}; n groups.  One atomic per CTA.
+__global__ void __launch_bounds__(kThreads) k_locks_held(const uint32_t* bits, const uint2* cnt2, uint64_t n, unsigned long long* out) {
+  __shared__ uint32_t wsum[kThreads / 32];
+  uint32_t held = 0;
+  const uint64_t m = bits ? (n + 31) / 32 : n;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t)gridDim.x * blockDim.x) {
+    if (bits) held += __popc(__ldcg(bits + i));
+    else { const uint2 v = __ldcg(cnt2 + i); held += (v.x | v.y) != 0; }
+  }
+  held = __reduce_add_sync(0xffffffffu, held);
+  if (lane_id() == 0) wsum[threadIdx.x / 32] = held;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long sum = 0;
+    for (uint32_t w = 0; w < kThreads / 32; w++) sum += wsum[w];
+    if (sum) atomicAdd(out, sum);
+  }
+}
+#endif
 
 }  // namespace dint

@@ -15,8 +15,14 @@
 // (p+2) % G, log records to those same three; G = 3 is exactly the reference.
 //
 // Statistics go to a Sink: begin(type) when a transaction starts, commit(type) when one commits, lock_reply(type) for
-// every absorbed reply to a TATP kAcquireLock.  One absorb finishes at most one transaction, starts at most one and
-// sees at most two lock replies, which the device sink relies on.
+// every absorbed reply to a TATP kAcquireLock.  One step (an absorb, then an emit) finishes at most one transaction,
+// starts at most one and sees at most two lock replies, which the device sink relies on.
+//
+// Draining (Cfg::drain): a client that finishes a transaction while the drain word is set counts the commit and goes
+// IDLE (txn == kIdle) instead of starting the next one.  An idle client emits and absorbs nothing; once the drain word
+// is clear again it begins its next transaction in the emit step, then emits that transaction's first records.  Every
+// draw happens in *_begin, so a drain changes when a client's transactions run, never which.  A round in which no
+// client emits a record is the end of a drain: nobody serves or counts it.
 //
 // Under nvcc the kernels of the on-GPU clients follow (one thread per client; see the comment above them).
 #pragma once
@@ -50,6 +56,9 @@ TXN_HD float fadd(float a, float b) {
 
 constexpr uint32_t kMaxRecords = 9;      // records one client emits in one round (SmallBank: 3 written rows x 3 holders)
 constexpr uint32_t kSeedBase = 0xdeadbeefu;   // client_udp_shard.cc:1121: seed = 0xdeadbeef + gid
+// txn of an idle client: never a transaction type (0 is X_GET_SUB / B_AMALGAMATE, and zero-filled storage is the initial
+// state)
+constexpr uint8_t kIdle = 0xFF;
 
 // ================================================ TATP ==============================================
 // wire: {ord@0, type@1, table@2, key@3, val@11[40], ver@51}  (tatp/udp/net.h:57-65)
@@ -92,6 +101,7 @@ struct Cfg {
   uint32_t G;              // shards
   uint32_t keys;           // tatp: kSubscriberNum; smallbank: kAccountNum
   uint32_t hot;            // smallbank: kHotAccountNum
+  uint32_t drain;          // != 0: a client that finishes a transaction goes idle instead of starting the next
 };
 TXN_HD uint32_t prim(const Cfg& w, uint64_t key) { return (uint32_t)(key % w.G); }
 
@@ -188,7 +198,8 @@ TXN_HD void tatp_begin(const Cfg& w, TatpClient& c, Sink& sink) {
 template <class Sink>
 TXN_HD void tatp_finish(const Cfg& w, TatpClient& c, bool committed, Sink& sink) {
   if (committed) sink.commit(c.txn);
-  tatp_begin(w, c, sink);
+  if (w.drain) c.txn = kIdle;
+  else tatp_begin(w, c, sink);
 }
 
 TXN_HD uint64_t k_sub(const TatpClient& c) { return c.s_id; }
@@ -199,10 +210,15 @@ TXN_HD void mk(TMsg& m, uint8_t type, uint8_t table, uint64_t key) {
   m.b[1] = type; m.b[2] = table; put64(m.b + 3, key);
 }
 
-// one protocol step of one client
-TXN_HD void tatp_emit(const Cfg& w, TatpClient& c, Out& o) {
+// one protocol step of one client; an idle client begins its next transaction first unless the clients drain
+template <class Sink>
+TXN_HD void tatp_emit(const Cfg& w, TatpClient& c, Out& o, Sink& sink) {
   const uint32_t n0 = o.n;
   o.n0 = n0;
+  if (c.txn == kIdle) {
+    if (w.drain) { c.n_out = 0; return; }
+    tatp_begin(w, c, sink);
+  }
   TMsg m;
   switch (c.txn) {
     case X_GET_SUB: mk(m, T_READ, TB_SUB, k_sub(c)); o.push(m, prim(w, k_sub(c)), false); break;                 // :177-199
@@ -291,6 +307,7 @@ TXN_HD bool tatp_lock_refused(uint8_t type) { return type == T_REJECT_LOCK || ty
 // r: the replies to the client's records of the last tatp_emit, in the same order
 template <class Sink>
 TXN_HD void tatp_absorb(const Cfg& w, TatpClient& c, const uint8_t* r, Sink& sink) {
+  if (c.txn == kIdle) return;
   switch (c.txn) {
     case X_GET_SUB: tatp_finish(w, c, true, sink); break;
     case X_GET_ACC: tatp_finish(w, c, tatp_type(r, 0) == T_GRANT_READ, sink); break;
@@ -459,12 +476,18 @@ TXN_HD void sb_begin(const Cfg& w, SbClient& c, Sink& sink) {
 template <class Sink>
 TXN_HD void sb_finish(const Cfg& w, SbClient& c, bool ok, Sink& sink) {
   if (ok) sink.commit(c.txn);
-  sb_begin(w, c, sink);
+  if (w.drain) c.txn = kIdle;
+  else sb_begin(w, c, sink);
 }
 
-TXN_HD void sb_emit(const Cfg& w, SbClient& c, Out& o) {
+template <class Sink>
+TXN_HD void sb_emit(const Cfg& w, SbClient& c, Out& o, Sink& sink) {
   const uint32_t n0 = o.n;
   o.n0 = n0;
+  if (c.txn == kIdle) {
+    if (w.drain) { c.n_out = 0; return; }
+    sb_begin(w, c, sink);
+  }
   switch (c.phase) {
     case SP_ACQ:
       for (int i = 0; i < c.n_rows; i++) {
@@ -504,6 +527,7 @@ TXN_HD int sb_next_granted(const SbClient& c, int from) {
 }
 template <class Sink>
 TXN_HD void sb_absorb(const Cfg& w, SbClient& c, const uint8_t* r, Sink& sink) {
+  if (c.txn == kIdle) return;
   switch (c.phase) {
     case SP_ACQ: {
       bool all = true;
@@ -591,7 +615,7 @@ struct DevClients {
 
 constexpr uint32_t kDevStats = 17;   // words of DevClients::stats
 
-// one absorb starts at most one transaction, commits at most one and sees at most two lock replies
+// one step starts at most one transaction, commits at most one and sees at most two lock replies
 struct DevSink {
   int began, done;
   uint32_t lock[3];             // lock replies, of them kRejectLock, kRejectLockSameKey
@@ -616,12 +640,12 @@ __global__ void __launch_bounds__(dint::kThreads, 1) k_txn_step(const DevClients
       TatpClient& c = ((TatpClient*)d.cl)[id];
       if (first) { c.seed = (uint64_t)kSeedBase + d.gid0 + id; tatp_begin(d.w, c, sink); }
       else tatp_absorb(d.w, c, resp + (size_t)d.off[id] * MSG, sink);
-      tatp_emit(d.w, c, o);
+      tatp_emit(d.w, c, o, sink);
     } else {
       SbClient& c = ((SbClient*)d.cl)[id];
       if (first) { c.seed = (uint64_t)kSeedBase + d.gid0 + id; sb_begin(d.w, c, sink); }
       else sb_absorb(d.w, c, resp + (size_t)d.off[id] * MSG, sink);
-      sb_emit(d.w, c, o);
+      sb_emit(d.w, c, o, sink);
     }
     d.cnt[id] = o.n;
     for (uint32_t i = 0; i < o.n; i++) atomicAdd(&s_own[o.dst[i]], 1u);

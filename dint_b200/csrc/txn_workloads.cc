@@ -4,7 +4,9 @@
 //
 // dint_txn_next() emits a round -- each client's records contiguous, in the order the reference pushes them per
 // shard -- plus the destination shard of every record; dint_txn_feed() hands the replies back in the same layout and
-// advances every client's state machine.
+// advances every client's state machine.  dint_txn_set_draining() lets the clients finish the transactions they are in
+// and start no new ones; an empty round is the end of such a drain, after which dint_txn_set_shards() may move them
+// to another shard count.
 #include <cstdint>
 #include <cstring>
 #include <vector>
@@ -58,14 +60,30 @@ void dint_txn_destroy(dint_txn* w) { delete w; }
 uint32_t dint_txn_max_round(const dint_txn* w) { return w->n_clients * kMaxRecords; }
 
 // emits one round; returns the number of wire records.  req: capacity dint_txn_max_round() records;
-// dst[i] = destination shard of record i.
+// dst[i] = destination shard of record i.  An empty round (the end of a drain) is not counted.
 uint64_t dint_txn_next(dint_txn* w, void* req, uint8_t* dst) {
   Out o{(uint8_t*)req, dst, 0, 0, w->kind == 4 ? (uint32_t)TM : (uint32_t)SMSZ};
-  if (w->kind == 4) for (auto& c : w->tc) tatp_emit(w->w, c, o);
-  else for (auto& c : w->sc) sb_emit(w->w, c, o);
+  if (w->kind == 4) for (auto& c : w->tc) tatp_emit(w->w, c, o, *w);
+  else for (auto& c : w->sc) sb_emit(w->w, c, o, *w);
   w->st_requests += o.n;
-  w->st_rounds++;
+  if (o.n) w->st_rounds++;
   return o.n;
+}
+// on != 0: a client that finishes its transaction goes idle; 0: idle clients begin again at the next dint_txn_next
+void dint_txn_set_draining(dint_txn* w, int on) { w->w.drain = on ? 1u : 0u; }
+// the clients mid-transaction (not idle)
+uint32_t dint_txn_busy(const dint_txn* w) {
+  uint32_t n = 0;
+  if (w->kind == 4) for (const auto& c : w->tc) n += c.txn != kIdle;
+  else for (const auto& c : w->sc) n += c.txn != kIdle;
+  return n;
+}
+// address every later record with key % G: only between transactions (busy == 0), G = 1 or 3..8.  0, or -22
+// (EINVAL) with nothing changed.
+int dint_txn_set_shards(dint_txn* w, uint32_t G) {
+  if (G == 0 || G == 2 || G > 8 || dint_txn_busy(w) != 0) return -22;
+  w->w.G = G;
+  return 0;
 }
 void dint_txn_feed(dint_txn* w, const void* resp) {
   const uint8_t* r = (const uint8_t*)resp;

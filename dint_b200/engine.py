@@ -76,10 +76,10 @@ _lib = None
 # every symbol include/dint_b200.h declares
 ABI_SYMBOLS = [
     "dint_msg_size", "dint_default_cfg", "dint_create", "dint_destroy", "dint_populate", "dint_load",
-    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_cluster_reshard", "dint_reshard_times", "dint_cluster_rebuild", "dint_cluster_image_open_rebuild", "dint_rebuild_times", "dint_cluster_clients_rebind", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
+    "dint_submit", "dint_submit_device", "dint_route_owner", "dint_route_partition", "dint_route_unpermute", "dint_route_tile_records", "dint_route_dispatch", "dint_route_combine", "dint_p2p_wait", "dint_p2p_signal", "dint_shard_create", "dint_shard_destroy", "dint_shard_submit_many", "dint_shard_submit_host", "dint_shard_submit_many_v", "dint_shard_flags", "dint_cluster_create", "dint_cluster_populate", "dint_cluster_submit", "dint_cluster_engine", "dint_cluster_size", "dint_cluster_overflow_retries", "dint_shard_recover", "dint_cluster_destroy", "dint_clients_create", "dint_clients_create_cfg", "dint_clients_run", "dint_clients_stats", "dint_clients_stats_all", "dint_clients_peek", "dint_clients_destroy", "dint_txn_clients_create", "dint_txn_clients_run", "dint_txn_clients_stats", "dint_txn_clients_peek", "dint_txn_clients_times", "dint_txn_clients_lock_stats", "dint_txn_clients_destroy", "dint_cluster_clients_create", "dint_cluster_clients_run", "dint_cluster_clients_stats", "dint_cluster_clients_peek", "dint_cluster_clients_times", "dint_cluster_clients_destroy", "dint_snapshot_create", "dint_snapshot_restore", "dint_snapshot_destroy", "dint_image_save", "dint_image_open", "dint_cluster_image_save", "dint_cluster_image_open", "dint_image_times", "dint_cluster_reshard", "dint_reshard_times", "dint_cluster_rebuild", "dint_cluster_image_open_rebuild", "dint_rebuild_times", "dint_cluster_clients_rebind", "dint_cluster_reshard_txn", "dint_txn_clients_drain", "dint_txn_clients_rebind", "dint_sync", "dint_kv_get", "dint_store_cache_set", "dint_store_cache_stats", "dint_tatp_cache_set", "dint_tatp_chain", "dint_tatp_cache_stats", "dint_smallbank_cache_set", "dint_smallbank_cache_stats", "dint_kv_count", "dint_lock_state", "dint_lock_holder",
     "dint_lock_slot", "dint_dump_log", "dint_log_entry_size", "dint_get_stats", "dint_reset_stats",
     "dint_profile", "dint_kernel_times", "dint_last_error", "dint_host_alloc", "dint_host_free",
-    "dint_test_fasthash64", "dint_test_fastmod", "dint_test_rebuild_source", "dint_test_host_slices",
+    "dint_test_fasthash64", "dint_test_fastmod", "dint_test_rebuild_source", "dint_test_txn_reshard_dests", "dint_test_host_slices",
 ]
 
 
@@ -136,6 +136,8 @@ def lib():
     L.dint_txn_clients_times.restype = i32; L.dint_txn_clients_times.argtypes = [vp, C.POINTER(C.c_double)]
     L.dint_txn_clients_lock_stats.restype = i32; L.dint_txn_clients_lock_stats.argtypes = [vp, C.POINTER(u64)]
     L.dint_txn_clients_destroy.restype = None; L.dint_txn_clients_destroy.argtypes = [vp]
+    L.dint_txn_clients_drain.restype = i32; L.dint_txn_clients_drain.argtypes = [vp, u32, C.POINTER(u32)]
+    L.dint_txn_clients_rebind.restype = i32; L.dint_txn_clients_rebind.argtypes = [vp, vp]
     L.dint_cluster_clients_create.restype = i32; L.dint_cluster_clients_create.argtypes = [vp, C.POINTER(DintClientsCfg), C.POINTER(vp)]
     L.dint_cluster_clients_run.restype = i32; L.dint_cluster_clients_run.argtypes = [vp, u32]
     L.dint_cluster_clients_stats.restype = i32; L.dint_cluster_clients_stats.argtypes = [vp, C.POINTER(u64)]
@@ -152,6 +154,7 @@ def lib():
     L.dint_image_times.restype = i32; L.dint_image_times.argtypes = [C.POINTER(C.c_double)]
     L.dint_cluster_reshard.restype = i32; L.dint_cluster_reshard.argtypes = [vp, i32, C.POINTER(i32), u64, C.POINTER(vp)]
     L.dint_reshard_times.restype = i32; L.dint_reshard_times.argtypes = [C.POINTER(C.c_double)]
+    L.dint_cluster_reshard_txn.restype = i32; L.dint_cluster_reshard_txn.argtypes = [vp, i32, C.POINTER(i32), u64, C.POINTER(vp)]
     L.dint_cluster_rebuild.restype = i32; L.dint_cluster_rebuild.argtypes = [vp, u32]
     L.dint_cluster_image_open_rebuild.restype = i32
     L.dint_cluster_image_open_rebuild.argtypes = [C.c_char_p, i32, C.POINTER(i32), u64, C.POINTER(u32), C.POINTER(vp)]
@@ -186,6 +189,7 @@ def lib():
     L.dint_test_fasthash64.restype = u64; L.dint_test_fasthash64.argtypes = [u64, i32]
     L.dint_test_fastmod.restype = u32; L.dint_test_fastmod.argtypes = [u64, u32]
     L.dint_test_rebuild_source.restype = i32; L.dint_test_rebuild_source.argtypes = [u64, u32, u32]
+    L.dint_test_txn_reshard_dests.restype = u32; L.dint_test_txn_reshard_dests.argtypes = [u64, u32, u32, u32]
     _lib = L
     return L
 
@@ -779,6 +783,20 @@ class GpuCluster:
         cl.kind, cl.msg, cl.G, cl.cfg, cl.h = self.kind, self.msg, n_shards, self.cfg, h
         return cl
 
+    def reshard_txn(self, n_shards, devices=None, max_batch=0):
+        """A new tatp / smallbank cluster of `n_shards` shards (1 or 3..8) on which every row sits on its replicas under
+        the new placement, copied with its version from the key's old primary (dint_cluster_reshard_txn).  Lock state,
+        the log ring and statistics start empty, and no lock may be held: drain the GpuTxnClients first.  This cluster
+        is not changed and stays usable.  devices / max_batch as for GpuCluster; peak device memory is both clusters."""
+        dv = (C.c_int * n_shards)(*devices) if devices is not None else None
+        h = C.c_void_p()
+        rc = lib().dint_cluster_reshard_txn(self.h, n_shards, dv, max_batch, C.byref(h))
+        if rc != 0:
+            raise DintError(rc, f"dint_cluster_reshard_txn({KIND_NAMES[self.kind]}, {self.G} -> {n_shards})")
+        cl = GpuCluster.__new__(GpuCluster)
+        cl.kind, cl.msg, cl.G, cl.cfg, cl.h = self.kind, self.msg, n_shards, self.cfg, h
+        return cl
+
     def engine(self, shard):
         """A non-owning Engine view of one shard (state inspection)."""
         e = Engine.__new__(Engine)
@@ -865,6 +883,25 @@ class GpuTxnClients:
         if rc != 0:
             raise DintError(rc, "dint_txn_clients_peek")
         return rq[: nn.value * self.msg], dst[: nn.value], rs[: nl.value * self.msg]
+
+    def drain(self, max_rounds=64):
+        """Serve rounds until every client has finished the transaction it was in and started no new one; returns the
+        rounds served (dint_txn_clients_drain).  The clients stay idle until the next run(), peek() or stats(), which
+        resumes them, possibly on another cluster (rebind)."""
+        n = C.c_uint32(0)
+        rc = lib().dint_txn_clients_drain(self.h, max_rounds, C.byref(n))
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_drain")
+        return int(n.value)
+
+    def rebind(self, cluster):
+        """Move drained clients (or clients that have never run) to `cluster`, a GpuCluster of the same kind (e.g. from
+        GpuCluster.reshard_txn): each client's state and the counters carry over (dint_txn_clients_rebind).  The old
+        cluster may then be closed."""
+        rc = lib().dint_txn_clients_rebind(self.h, cluster.h)
+        if rc != 0:
+            raise DintError(rc, "dint_txn_clients_rebind")
+        self.cluster = cluster
 
     def times(self):
         """Rounds timed by run(), their host wall time and the CUDA-event time of their device work (rank 0), in s."""

@@ -35,6 +35,11 @@ def lib():
         L.dint_txn_feed.argtypes = [C.c_void_p, C.c_void_p]
         L.dint_txn_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
         L.dint_txn_lock_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.dint_txn_set_draining.argtypes = [C.c_void_p, C.c_int]
+        L.dint_txn_busy.restype = C.c_uint32
+        L.dint_txn_busy.argtypes = [C.c_void_p]
+        L.dint_txn_set_shards.restype = C.c_int
+        L.dint_txn_set_shards.argtypes = [C.c_void_p, C.c_uint32]
         _lib = L
     return _lib
 
@@ -53,6 +58,29 @@ class TxnWorkload:
         self._req = np.empty(cap * self.msg, dtype=np.uint8)
         self._dst = np.empty(cap, dtype=np.uint8)
         self._n = 0
+        self._draining = False
+
+    @property
+    def draining(self):
+        """True: a client that finishes its transaction goes idle instead of starting the next; next() then returns an
+        empty round once every client is idle.  False again: idle clients begin at the next next()."""
+        return self._draining
+
+    @draining.setter
+    def draining(self, on):
+        lib().dint_txn_set_draining(self.h, 1 if on else 0)
+        self._draining = bool(on)
+
+    def busy(self):
+        """The clients mid-transaction (not idle)."""
+        return int(lib().dint_txn_busy(self.h))
+
+    def set_shards(self, n_shards):
+        """Address every later record with key % n_shards (1 or 3..8).  Only between transactions: after a drain, when
+        busy() == 0."""
+        if lib().dint_txn_set_shards(self.h, n_shards) != 0:
+            raise ValueError(f"set_shards({n_shards}): {self.busy()} clients mid-transaction, or not 1 or 3..8 shards")
+        self.n_shards = n_shards
 
     def close(self):
         if self.h:

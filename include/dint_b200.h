@@ -555,6 +555,29 @@ int dint_cluster_image_open_rebuild(const char *dir, int n_gpus, const int *devi
 int dint_rebuild_times(double out[3]);
 
 /*
+ * Re-sharding tatp / smallbank clusters: re-placing every row on its replicas under another shard count.
+ *   dint_cluster_reshard_txn: a new tatp or smallbank cluster of n_gpus shards (1 or 3..8), built as
+ *     dint_cluster_create(kind, src's cfg, n_gpus, devices, max_batch) would build it.  Each shard j holds, for every key
+ *     it replicates under the new placement (j is (k % n_gpus + i) % n_gpus for some i in 0..2), the row of the key's
+ *     old primary, shard k % G of src: its value and version.  At a drained point (dint_txn_clients_drain, or population
+ *     and nothing since) every replica of a key holds the same row, so the new cluster answers every later transaction
+ *     as src would under the new placement.  One fixed source per key makes the result independent of launch order.
+ *     Only FULL rows move; deleted rows stay absent.  Each table is at least as large as dint_cluster_create makes it,
+ *     and large enough to keep its rows at <= 35 % load.
+ *     Not moved: lock words, holder keys and SmallBank counters start free (the call requires them free, so nothing is
+ *     lost); the log ring starts empty (nothing reads it, and for G > 3 arrival order has no meaning on another shard);
+ *     statistics start at zero.  src is read, never changed, and stays usable; it is synchronised first.  A source shard
+ *     on another GPU is read over peer memory.  Peak device memory is src plus the new cluster.  The call is timed in
+ *     dint_reshard_times.
+ *     DINT_EINVAL, *out = NULL and src unchanged, with the reason in dint_last_error(): kinds other than tatp and
+ *     smallbank (their call is dint_cluster_reshard); DINT_CFG_TATP_EBPF and DINT_CFG_SMALLBANK_EBPF (as for
+ *     dint_cluster_rebuild); n_gpus of 0, 2 or more than 8; devices neither all distinct nor all the same; and any held
+ *     lock (a TATP lock bit, a SmallBank counter not {0, 0}) on any source shard, naming the shard and the count: clients
+ *     are mid-transaction, drain them first.
+ */
+int dint_cluster_reshard_txn(dint_cluster *src, int n_gpus, const int *devices, uint64_t max_batch, dint_cluster **out);
+
+/*
  * lock_2pl, lock_fasst, log_server and store closed-loop clients ON the GPU (SURVEY.md section 8(f) rank 2).  The
  * reference's clients are Caladan uthreads on other machines (lock_2pl/caladan/client.cc:181-230,
  * lock_fasst/caladan/client.cc:183-280, store/caladan/client_udp.cc:135-208; trace shapes lock_2pl/caladan/
@@ -613,6 +636,19 @@ void dint_clients_destroy(dint_clients *c);
  *     their destination shards) and the replies absorbed last (n_last records); buffers of n_clients * 9 records.
  *   dint_txn_clients_times: rounds timed by run, their host wall time (s) and the CUDA-event time (s) of their device
  *     work on rank 0's stream; the difference is the host time the round-trip leaves exposed.
+ *   dint_txn_clients_drain (blocking): serve rounds in draining mode -- every client finishes the transaction it is in
+ *     and starts no new one -- until the pending round is empty.  *rounds receives the rounds served (they count in
+ *     stats; no transaction starts during a drain).  A drain ends within L + 1 emissions, L the longest transaction in
+ *     rounds (TATP 7, SmallBank 5): at most L rounds served.  Returns 0 when drained, DINT_EPROTO as run does, and
+ *     DINT_EINVAL with the count of clients still mid-transaction when records are pending after max_rounds (the
+ *     clients then continue at the next run).  Drained clients stay idle until the next run, peek or stats call, which
+ *     resumes them: every idle client begins its next transaction and emits on the cluster it is bound to.  Each
+ *     client's transaction stream is the one it would have run without the drain, only later.
+ *   dint_txn_clients_rebind: move drained clients, or clients that have never emitted, to cluster c (e.g. the result of
+ *     dint_cluster_reshard_txn): each client's state moves to c's ranks in contiguous blocks, across devices if needed,
+ *     and the counters carry over.  Afterwards the clients no longer reference the old cluster, which may be destroyed:
+ *     its dint_txn_clients attachment (the one dint_cluster_rebuild refuses) moves to c.  DINT_EINVAL, the clients
+ *     unchanged: clients mid-transaction, a cluster of another kind, and every cluster dint_txn_clients_create refuses.
  * The first round is emitted by the first run, peek or stats call.
  */
 typedef struct dint_txn_clients dint_txn_clients;
@@ -621,6 +657,8 @@ int dint_txn_clients_run(dint_txn_clients *t, uint32_t rounds);
 int dint_txn_clients_stats(dint_txn_clients *t, uint64_t out[19]);
 int dint_txn_clients_peek(dint_txn_clients *t, void *next_req, uint8_t *next_dst, uint64_t *n_next, void *last_resp, uint64_t *n_last);
 int dint_txn_clients_times(dint_txn_clients *t, double out[3]);
+int dint_txn_clients_drain(dint_txn_clients *t, uint32_t max_rounds, uint32_t *rounds);
+int dint_txn_clients_rebind(dint_txn_clients *t, dint_cluster *c);
 /* The lock counters of tatp/caladan/client_lock.cc, summed over the clients (synchronises): [0] kAcquireLock replies
  * absorbed (lock_cnt, :718,1056,1309,1583), [1] of them kRejectLock = refused through false sharing
  * (reject_sharing_cnt), [2] kRejectLockSameKey = refused by a holder of the same key (reject_same_key_cnt); the two
@@ -685,6 +723,9 @@ uint32_t dint_test_fastmod(uint64_t n, uint32_t d);
 /* the source shard dint_cluster_rebuild copies key's rows from in a G-shard cluster that lost the shards of lost_mask,
  * or -1 when every replica of the key is lost (or G is outside 1..8) */
 int dint_test_rebuild_source(uint64_t key, uint32_t G, uint32_t lost_mask);
+/* the bit mask of shards dint_cluster_reshard_txn gives key's row when it re-places a G-shard cluster onto G2 shards and
+ * reads source shard src: (k % G2 + i) % G2 for i = 0..2 when src == k % G, else 0 (0 also for G or G2 outside 1..8) */
+uint32_t dint_test_txn_reshard_dests(uint64_t key, uint32_t G, uint32_t G2, uint32_t src);
 /* test hook: the slice sizes dint_submit cuts a call of n requests into (host logic, no GPU needed);
  * returns the number of slices, writes the first `cap` of them */
 uint32_t dint_test_host_slices(uint64_t n, uint32_t min_slice, uint32_t max_slice, int ramp_up, uint32_t *out, uint32_t cap);
