@@ -47,16 +47,31 @@ def build(force=False, verbose=False):
             all(os.path.exists(p) for p in (LIB, WL_LIB, UDP_SERVER)):
         return LIB                    # a read-only tree: use the libraries it was built with
     os.makedirs(LIBDIR, exist_ok=True)
-    cu_src = _sources((".cu", ".cuh", ".h"))
+    headers = _sources((".cuh", ".h"))
+    units = _sources((".cu",))
     # a tagged library that exists is used as built: it may be a frozen build of another commit for an A/B run
-    if (force or _newer(LIB, cu_src)) and not (_TAG and os.path.exists(LIB)):
+    if (force or _newer(LIB, units + headers)) and not (_TAG and os.path.exists(LIB)):
         nvcc = find_nvcc()
         if nvcc is None:
             raise RuntimeError("nvcc not found: cannot build libdint_b200.so (there is no CPU fallback)")
         # DINT_NVCC_DEFINES: extra -D flags for A/B builds of a development variant (none exist at the moment)
-        cmd = [nvcc] + NVCC_FLAGS + os.environ.get("DINT_NVCC_DEFINES", "").split() + (["-Xptxas", "-v"] if verbose else []) + \
-              ["-o", LIB, os.path.join(CSRC, "engine.cu")]
-        subprocess.run(cmd, check=True)
+        flags = [f for f in NVCC_FLAGS if f != "-shared"] + os.environ.get("DINT_NVCC_DEFINES", "").split() + \
+            (["-Xptxas", "-v"] if verbose else [])
+        # one object per unit (each kernel is compiled in exactly one), compiled in parallel; an object is rebuilt when
+        # its unit or any header is newer.  Tagged builds keep tagged objects.
+        objs, jobs = [], []
+        for src in units:
+            obj = os.path.join(LIBDIR, os.path.basename(src)[:-3] + (f"_{_TAG}" if _TAG else "") + ".o")
+            objs.append(obj)
+            if force or _newer(obj, [src] + headers):
+                jobs.append((subprocess.Popen([nvcc] + flags + ["-c", "-o", obj, src]), obj))
+        failed = [obj for proc, obj in jobs if proc.wait() != 0]
+        for obj in failed:
+            if os.path.exists(obj):
+                os.remove(obj)
+        if failed:
+            raise RuntimeError("nvcc failed: " + ", ".join(os.path.basename(o) for o in failed))
+        subprocess.run([nvcc] + NVCC_FLAGS + ["-o", LIB] + objs, check=True)
     wl_src = [os.path.join(CSRC, "workloads.cc"), os.path.join(CSRC, "txn_workloads.cc")]
     if os.path.exists(wl_src[0]) and (force or _newer(WL_LIB, wl_src + _sources((".h", ".cuh")))):
         subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wall", "-o", WL_LIB] + wl_src, check=True)

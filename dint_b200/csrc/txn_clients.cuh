@@ -1,5 +1,5 @@
 // txn_clients.cuh -- the TATP and SmallBank closed-loop client state machines, stated ONCE for the host drivers
-// (txn_workloads.cc, g++, libdint_wl.so) and the clients that run on the GPU (engine.cu, nvcc, dint_txn_clients_*).
+// (txn_workloads.cc, g++, libdint_wl.so) and the clients that run on the GPU (clients.cu, nvcc, dint_txn_clients_*).
 //
 // The reference: tatp/caladan/client_udp_shard.cc:177-1184 (seven transaction types, mix 35/35/10/2/14/2/2,
 // tatp/udp/tatp.h:57-63) and smallbank/caladan/client_udp_shard.cc:169-1300 (six types, mix 15/15/15/25/15/15,
